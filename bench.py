@@ -53,7 +53,7 @@ CONFIGS = {
                                '(BASELINE configs[4])'),
 }
 EMB_DIM = 16      # of the headline config (CIN_FLOP_PER_ROW below)
-# algorithmic work per row, SURVEY.md 8(d) / DESIGN.md section 5
+# algorithmic work per row, SURVEY.md 8(d)
 CIN_FLOP_PER_ROW = 2 * EMB_DIM * sum(l * k for l, k in zip(CIN_SIZES, (26 * 26, 26 * 64, 26 * 64)))  # 16 400 384
 CIN_BYTES_PER_ROW = 4 * F_FIELDS + 4 * F_FIELDS * EMB_DIM + 4 * (64 + 64 + 128)                        # ids + rows + pooled
 
@@ -72,10 +72,12 @@ def parse_args():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--cin-precision', type=int, default=0)
     ap.add_argument('--no-graph', action='store_true', help='eager launches instead of the CUDA-graph replay of the train step')
-    ap.add_argument('--cin-exp', type=int, default=0,
-                    help='profiling only: experiment build of the CIN backward kernels (cin_tc.cu), 0 = product kernels')
     ap.add_argument('--id-dist', default='uniform', choices=['uniform', 'zipf'],
                     help="categorical id distribution of the synthetic batches (the headline is 'uniform')")
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the device-resident timed steps (the headline loop, before the end-to-end loop), write '
+                         'what the last of them computed (its predictions, the accumulated loss, a fixed seeded sample '
+                         'of every parameter) as DIR/<name>.npy; needs --steps >= 1')
     return ap.parse_args()
 
 
@@ -98,7 +100,7 @@ def make_config(name='xdeepfm', cin_precision=0):
 
 def reference_config(name):
     """The same configuration for the CPU arm WITHOUT importing the product package (whose import loads the CUDA
-    library): the reference's own ModelConfig() defaults, as dumped from /root/reference by
+    library): the reference project's own ModelConfig() defaults, as dumped by
     tests/golden/make_reference_golden.py, overlaid with the bench overrides.  oracle/model_ref.py reads dicts."""
     with open(os.path.join(ROOT, 'tests', 'golden', 'reference_modelconfig.json')) as f:
         conf = dict(json.load(f)['defaults'])
@@ -130,7 +132,7 @@ def synth_batches(n_batches, batch, vocab, seed, id_dist='uniform', pin=True):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -200,7 +202,8 @@ def measured_peaks():
             p = json.load(f)
         return {'hbm_gbs': p['hbm_gbs'], 'bf16_tflops': p['bf16_tflops'],
                 'bf16_tflops_sustained': p.get('bf16_tflops_sustained', p['bf16_tflops']), 'source': 'measured'}
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0, 'source': 'fallback'}
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- not measured values
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0, 'source': 'datasheet'}
 
 
 def cpu_baseline(args, conf, steps=None):
@@ -363,32 +366,58 @@ def time_cin_kernel(model, cat, peaks):
     dt_b = _timed_alone(bwd, flush)
     t.grad.zero_()                                     # the probe's gradients must not leak into training
     mode = N.lib.dtb_cin_resolved_precision(F_FIELDS, EMB_DIM, sizes_c, 3, 0, precision)     # what 'auto' runs for this shape
-    tc = mode in (2, 3, 4)
     tf = b * CIN_FLOP_PER_ROW / dt / 1e12
-    kname = {4: 'cin_tc2_fwd_kernel', 2: 'cin_tc_fwd_kernel', 3: 'cin_tc_fwd_kernel'}.get(mode)
-    traffic = None
-    tpath = os.path.join(ROOT, 'profiles', 'r2_cin_tc_traffic.json')
-    if kname and os.path.exists(tpath) and b == 65536:
-        with open(tpath) as f:
-            tj = json.load(f).get(kname)            # ncu --set full capture of this kernel at this shape (training mode)
-        if tj:
-            traffic = tj['dram_bytes_read'] + tj['dram_bytes_write']
     return {'bound': 'tensor', 'achieved': tf, 'peak': peaks['bf16_tflops'], 'unit': 'TFLOP/s',
-            'frac': tf / peaks['bf16_tflops'], 'traffic': traffic,
-            'kernel': {4: 'cin_tc2_fwd_kernel (tcgen05, ONE pass on power-of-two-scaled fp16 operands, two threads per GEMM row)',
-                       2: 'cin_tc_fwd_kernel (tcgen05, bf16x3 split: 3 tensor passes per algorithmic FLOP)',
-                       3: 'cin_tc_fwd_kernel (tcgen05, one bf16 pass)'}.get(mode, 'cin_fwd (any-shape formulation, dense_tc GEMMs)'),
-            'ms': dt * 1e3, 'algorithmic_flop_per_launch': b * CIN_FLOP_PER_ROW,
+            'frac': tf / peaks['bf16_tflops'], 'traffic': None,
+            'kernel': {1: 'cin_fwd (any-shape formulation: outer product in row chunks, bf16x3 wgmma GEMMs of dense_tc)',
+                       2: 'cin_wg_fwd_kernel (fused, wgmma with A from registers, bf16x3 split)',
+                       3: 'cin_wg_fwd_kernel (fused, wgmma, one bf16 pass)',
+                       4: 'cin_wg_fwd_kernel (fused, wgmma, one pass on power-of-two-scaled fp16 operands)'}[mode],
+            'cin_precision': mode, 'ms': dt * 1e3, 'algorithmic_flop_per_launch': b * CIN_FLOP_PER_ROW,
             'algorithmic_bytes_per_launch': b * CIN_BYTES_PER_ROW,
-            'executed_tensor_tflops': tf * (3 if mode == 2 else 1),
+            'executed_tensor_tflops': tf * (3 if mode in (1, 2) else 1),
             'hbm_gbs_informational': b * CIN_BYTES_PER_ROW / dt / 1e9, 'peak_source': peaks['source'],
             'cin_backward': {'ms': dt_b * 1e3, 'algorithmic_tflops': 2 * b * CIN_FLOP_PER_ROW / dt_b / 1e12,
-                             'kernels': 'cin_tc2_dgrad_kernel + 3 x cin_tc2_wgrad_kernel' if mode == 4 else
-                                        'cin_tc_dgrad_kernel + 3 x cin_tc_wgrad_kernel'}}
+                             'kernels': 'cin_wg_dgrad_kernel + 3 x cin_wg_wgrad_kernel (fused, bf16x3)' if mode > 1 else
+                                        'cin_bwd (any-shape formulation, bf16x3 wgmma GEMMs of dense_tc)'}}
+
+
+DUMP_BUDGET_BYTES = 64 << 20
+DUMP_SAMPLE = 1 << 16          # elements kept of a parameter larger than this (fixed seeded positions)
+
+
+def collect_outputs(model, prob):
+    """What the last timed train step hands its caller, as host float32/float64 arrays: the batch predictions it returns,
+    the summed loss it accumulates, and the parameters it updated (a fixed, seeded sample of each large one)."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    out = {'predictions': prob.detach().float().cpu().numpy(), 'loss_sum': model._loss_acc.detach().double().cpu().numpy()}
+    for name, t in sorted(model.state_dict().items()):
+        if not torch.is_floating_point(t):
+            continue
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            pos = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+            flat = flat[pos.to(flat.device)]
+        out['param__' + name.replace('/', '__').replace('.', '_')] = flat.float().cpu().numpy()
+    total = sum(a.nbytes for a in out.values())
+    assert total <= DUMP_BUDGET_BYTES, f'dump of {total} bytes exceeds {DUMP_BUDGET_BYTES}'
+    return out
+
+
+def write_outputs(path, arrays):
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + '.npy'), a)
 
 
 def main():
     args = parse_args()
+    if args.dump_outputs and args.steps < 1:
+        sys.exit('--dump-outputs needs at least one timed step (--steps >= 1)')
     if args.impl == 'reference':
         run_reference(args)
         return
@@ -411,8 +440,6 @@ def main():
         args.batch = spec['batch']
     emb_dim = spec['dim']
     conf = make_config(args.config, args.cin_precision)
-    if args.cin_exp:
-        N.check(N.lib.dtb_cin_tc_set_variant(1 | (args.cin_exp << 12)), 'cin_tc_set_variant')
     cats = [CategoricalColumn(f'C{i + 1}', args.vocab, emb_dim) for i in range(F_FIELDS)]
     conts = [ContinuousColumn('input_continuous_all', [f'I{i + 1}' for i in range(N_DENSE)])]
     model = DeepModel('binary', 2, conf, cats, conts, seed=1234)
@@ -442,9 +469,11 @@ def main():
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item()) * 1e-3
 
+    last = {}
+
     def dev_step(s):
         c, d, y = devb[s % n_pool]
-        model.train_step(c, d, y)
+        last['prob'] = model.train_step(c, d, y)
 
     def e2e_step(s):
         c, d, y = host[s % n_pool]
@@ -459,6 +488,7 @@ def main():
     secs = timed(dev_step, args.steps)
     launches = N.lib.dtb_launch_count() - l0
     clocks = sampler.stop() if rank == 0 else None
+    dumped = collect_outputs(model, last['prob']) if args.dump_outputs and rank == 0 else None
     for s in range(2):
         e2e_step(s)
     secs_e2e = timed(e2e_step, args.steps)
@@ -493,11 +523,8 @@ def main():
             'metric': spec['metric'], 'value': rows / secs, 'unit': 'rows/s',
             'n_gpus': world, 'steps': args.steps, 'warmup': max(args.warmup, 3), 'ms_per_step': secs / args.steps * 1e3,
             'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-            'dtype': ('f32 storage and accumulation; CIN GEMMs: one tcgen05 pass on power-of-two-scaled fp16 operands (error ~2e-4 '
-                      'of the output scale); Dense GEMMs: bf16x3 split' if roof['kernel'].startswith('cin_tc2')
-                      else 'f32 (CIN GEMMs: bf16x3 split on tcgen05, fp32 accumulate)' if roof['kernel'].startswith('cin_tc_')
-                      else 'f32 (Dense GEMMs: bf16x3 split on tcgen05, fp32 accumulate)'),
-            'experiment_build': args.cin_exp or None,
+            'dtype': 'f32 (Dense and CIN GEMMs: bf16x3 split on wgmma, fp32 accumulate)' if roof.get('cin_precision', 2) in (1, 2)
+                     else f"f32 storage; CIN forward with a single tensor pass (precision code {roof['cin_precision']}), bf16x3 backward",
             'data': 'synthetic' if args.id_dist == 'uniform' else f'synthetic ({args.id_dist} ids: NOT the headline distribution)',
             'config': {'workload': spec['workload'], 'name': args.config,
                        'global_batch': args.batch * world, 'per_gpu_batch': args.batch, 'parallelism': f'dp{world}',
@@ -516,6 +543,8 @@ def main():
         if world == 1 and not args.no_cpu_baseline:
             base = cpu_baseline(args, reference_config(args.config))
             line['cpu_baseline'] = {k: base[k] for k in ('value', 'unit', 'cores', 'kind', 'sample')}
+        if dumped is not None:
+            write_outputs(args.dump_outputs, dumped)
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()

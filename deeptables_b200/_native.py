@@ -15,7 +15,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), 'include', 'deeptables_b200.h
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
-        f'{LIB_PATH} is missing: the sm_100a extension is not built. Run '
+        f'{LIB_PATH} is missing: the sm_90a extension is not built. Run '
         f'`python -c "import __graft_entry__ as g; g.build()"` (or `python deeptables_b200/build.py`) '
         f'from the repo root. There is no CPU fallback.')
 

@@ -1,9 +1,9 @@
-"""Build the sm_100a shared library in-tree (nvcc cross-compiles without a GPU).
+"""Build the sm_90a (H100) shared library in-tree (nvcc cross-compiles without a GPU).
 
     python deeptables_b200/build.py
 
 Produces deeptables_b200/_native/libdeeptables_b200.so -- the one artefact the ctypes binding
-(deeptables_b200/_native.py) loads.  The .so is git-ignored but travels to the GPU box.
+(deeptables_b200/_native.py) loads.  The .so and the object files are build products (git-ignored).
 """
 import glob
 import hashlib
@@ -16,7 +16,8 @@ CSRC = os.path.join(HERE, 'csrc')
 OUT_DIR = os.path.join(HERE, '_native')
 OUT = os.path.join(OUT_DIR, 'libdeeptables_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+GENCODE = ['-gencode', 'arch=compute_90a,code=sm_90a']
+FLAGS = GENCODE + ['-O3', '-lineinfo', '-std=c++17',
          '-Xcompiler', '-fPIC', '-DDTB_BUILD',
          '-shared'] + os.environ.get('NVCCFLAGS_EXTRA', '').split()
 
@@ -44,7 +45,7 @@ def build(force=False, verbose=True):
         return OUT
     if not os.path.exists(NVCC):
         if os.path.exists(OUT):
-            return OUT      # GPU box without a toolchain mismatch: use the shipped artefact
+            return OUT      # no toolchain here: use the library an earlier build left
         raise RuntimeError(f'nvcc not found at {NVCC} and no prebuilt {OUT}')
     objs = []
     procs = []
@@ -61,7 +62,7 @@ def build(force=False, verbose=True):
             raise RuntimeError(f'nvcc failed on {src}:\n{out.decode()}')
         if verbose and out.strip():
             sys.stderr.write(out.decode())
-    cmd = [NVCC, '-gencode', 'arch=compute_100a,code=sm_100a', '-shared', '-o', OUT] + objs      # no GEMM library: every kernel of the product is hand-written
+    cmd = [NVCC] + GENCODE + ['-shared', '-o', OUT] + objs      # no GEMM library: every kernel of the product is hand-written
     subprocess.check_call(cmd)
     with open(stamp, 'w') as f:
         f.write(fp)

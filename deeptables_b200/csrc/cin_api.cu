@@ -1,22 +1,23 @@
-// C-ABI entry points for CIN: shape validation and dispatch between the tensor-core kernel
-// (cin_tc.cu, product path) and the exact-fp32 any-shape formulation (cin_fp32.cu).
+// C-ABI entry points for CIN: shape validation and dispatch between the fused tensor-core forward (cin_wgmma.cu) and the
+// any-shape formulation (cin_fp32.cu: outer product in bounded chunks of batch rows, GEMMs on the wgmma kernels of
+// dense_tc.cu), and likewise between the two backwards.  Both forwards save the same activations.
 #include "dtb_common.cuh"
 #include "cin_shapes.h"
 #include "cin_impl.h"
 
 using namespace dtb;
 
-static bool use_tc(const CinShape& s, int precision) {
-  if (precision == DTB_CIN_FP32) return false;
-  return cin_tc_supported(s);
+static bool is_fused_tc(int precision) {
+  return precision == DTB_CIN_TC_BF16X3 || precision == DTB_CIN_TC_BF16X1 || precision == DTB_CIN_TC_F16X1;
 }
 
-// DTB_CIN_AUTO: single-pass fp16 tensor-core kernels where all three (forward, data gradient, weight gradient) take the
-// shape, else the bf16x3 tensor-core kernels, else the any-shape formulation.  Forward and backward of one step resolve
-// identically (same shape, same process-wide switches).
+// test hook (bit 16 of dtb_cin_tc_set_variant): the any-shape backward after a fused forward
+static int g_bwd_fp32 = 0;
+
+// auto: the fp32-grade bf16x3 fused forward where the shape fits it, else the any-shape formulation
 static int resolve_precision(const CinShape& s, int precision) {
-  if (precision == DTB_CIN_AUTO && cin_tc_f16_auto(s)) return DTB_CIN_TC_F16X1;
-  return precision;
+  if (precision != DTB_CIN_AUTO) return precision;
+  return cin_wg_supported(s) ? DTB_CIN_TC_BF16X3 : DTB_CIN_FP32;
 }
 
 extern "C" {
@@ -24,31 +25,32 @@ extern "C" {
 int dtb_cin_tc_supported(int F, int D, const int* layer_sizes_host, int n_layers, int direct) {
   CinShape s;
   if (!s.init(F, D, layer_sizes_host, n_layers, direct)) return 0;
-  return cin_tc_supported(s) ? 1 : 0;
+  return cin_wg_supported(s) ? 1 : 0;
 }
 
 int dtb_cin_resolved_precision(int F, int D, const int* layer_sizes_host, int n_layers, int direct, int precision) {
   CinShape s;
   if (!s.init(F, D, layer_sizes_host, n_layers, direct)) return DTB_ERR_INVALID_ARG;
-  precision = resolve_precision(s, precision);
-  if (precision == DTB_CIN_AUTO) return cin_tc_supported(s) ? DTB_CIN_TC_BF16X3 : DTB_CIN_FP32;
-  return precision;
+  return resolve_precision(s, precision);
 }
 
 size_t dtb_cin_saved_bytes(int B, int F, int D, const int* layer_sizes_host, int n_layers, int direct) {
   CinShape s;
   if (!s.init(F, D, layer_sizes_host, n_layers, direct) || B <= 0) return 0;
-  size_t a = cin_fp32_saved_bytes(s, B);
-  size_t b = cin_tc_supported(s) ? cin_tc_saved_bytes(s, B) : 0;
-  return a > b ? a : b;
+  return cin_fp32_saved_bytes(s, B);
 }
 
 size_t dtb_cin_workspace_bytes(int B, int F, int D, const int* layer_sizes_host, int n_layers, int direct,
                                int training) {
   CinShape s;
   if (!s.init(F, D, layer_sizes_host, n_layers, direct) || B <= 0) return 0;
-  size_t a = cin_fp32_workspace_bytes(s, B, training);
-  size_t b = cin_tc_supported(s) ? cin_tc_workspace_bytes(s, B, training) : 0;
+  const size_t a = cin_fp32_workspace_bytes(s, B, training);
+  size_t b = 0;
+  if (cin_wg_supported(s)) {
+    b = cin_wg_workspace_bytes(s);
+    const size_t c = training ? cin_wg_bwd_workspace_bytes(s, B) : 0;
+    b = b > c ? b : c;
+  }
   return a > b ? a : b;
 }
 
@@ -68,14 +70,13 @@ int dtb_cin_fwd(const int32_t* idx, const float* table, const int64_t* row_offse
   if (B <= 0) return DTB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   precision = resolve_precision(s, precision);
-  if (use_tc(s, precision)) {
-    const int single = precision == DTB_CIN_TC_BF16X1 || precision == DTB_CIN_TC_F16X1;
-    return cin_tc_fwd(s, idx, table, row_offsets, weights, bias, pooled, saved, workspace, workspace_bytes, B,
-                      act, single ? 1 : 3, precision == DTB_CIN_TC_F16X1 ? 1 : 0, status, st);
-  }
-  if (precision == DTB_CIN_TC_BF16X3 || precision == DTB_CIN_TC_BF16X1 || precision == DTB_CIN_TC_F16X1) {
-    set_error("dtb_cin_fwd: tensor-core path requested but shape unsupported (F=%d D=%d)", F, D);
-    return DTB_ERR_UNSUPPORTED;
+  if (is_fused_tc(precision)) {
+    if (!cin_wg_supported(s)) {
+      set_error("dtb_cin_fwd: tensor-core path requested but shape unsupported (F=%d D=%d)", F, D);
+      return DTB_ERR_UNSUPPORTED;
+    }
+    return cin_wg_fwd(s, idx, table, row_offsets, weights, bias, pooled, saved, workspace, workspace_bytes, B, act,
+                      precision - DTB_CIN_TC_BF16X3, status, st);
   }
   return cin_fp32_fwd(s, idx, table, row_offsets, weights, bias, pooled, saved, workspace, workspace_bytes, B,
                       act, status, st);
@@ -97,18 +98,15 @@ static int cin_bwd_impl(const int32_t* idx, const float* table, const int64_t* r
   }
   if (B <= 0) return DTB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  precision = resolve_precision(s, precision);
-  if (use_tc(s, precision))
-    return cin_tc_bwd(s, idx, table, row_offsets, weights, d_pooled, saved, grad_table, d_weights, d_bias,
-                      workspace, workspace_bytes, B, act, precision == DTB_CIN_TC_BF16X1 ? 1 : 3,
-                      precision == DTB_CIN_TC_F16X1 ? 1 : 0, phase, st);
-  if (precision == DTB_CIN_TC_BF16X3 || precision == DTB_CIN_TC_BF16X1 || precision == DTB_CIN_TC_F16X1) {
+  if (is_fused_tc(resolve_precision(s, precision)) && !cin_wg_supported(s)) {
     set_error("dtb_cin_bwd: tensor-core path requested but shape unsupported (F=%d D=%d)", F, D);
     return DTB_ERR_UNSUPPORTED;
   }
-  if (phase == 2) return DTB_OK;
+  if (is_fused_tc(resolve_precision(s, precision)) && !g_bwd_fp32)
+    return cin_wg_bwd(s, idx, row_offsets, weights, d_pooled, saved, grad_table, d_weights, d_bias, workspace,
+                      workspace_bytes, B, act, phase, st);
   return cin_fp32_bwd(s, idx, table, row_offsets, weights, d_pooled, saved, grad_table, d_weights, d_bias,
-                      workspace, workspace_bytes, B, act, st);
+                      workspace, workspace_bytes, B, act, phase, st);
 }
 
 int dtb_cin_bwd(const int32_t* idx, const float* table, const int64_t* row_offsets, const float* weights,
@@ -126,6 +124,11 @@ int dtb_cin_bwd_phase(const int32_t* idx, const float* table, const int64_t* row
   DTB_CHECK_ARG(phase == 1 || phase == 2, "phase must be 1 (embedding gradient) or 2 (weight gradient)");
   return cin_bwd_impl(idx, table, row_offsets, weights, d_pooled, saved, grad_table, d_weights, d_bias, workspace,
                       workspace_bytes, B, F, D, layer_sizes_host, n_layers, direct, act, precision, phase, stream);
+}
+
+int dtb_cin_tc_set_variant(int variant) {
+  g_bwd_fp32 = (variant >> 16) & 1;
+  return DTB_OK;
 }
 
 }  // extern "C"

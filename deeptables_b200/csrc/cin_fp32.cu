@@ -192,7 +192,7 @@ size_t cin_fp32_workspace_bytes(const CinShape& s, int B, int training) {
     bytes += (size_t)B * s.D * (s.F + s.sumL) * sizeof(float);          // x0t + T_k live in workspace
   } else {
     bytes += z;                                                         // dZ chunk
-    bytes += (size_t)bc * s.D * s.Lmax * sizeof(float);                 // dC
+    bytes += (size_t)B * s.D * s.sumL * sizeof(float);                  // dC_k of every row: phase 2 reads it
     bytes += 2 * (size_t)bc * s.D * s.Hmax * sizeof(float);             // dh ping-pong
     bytes += (size_t)bc * s.D * s.F * sizeof(float);                    // dx0t
   }
@@ -255,10 +255,12 @@ int cin_fp32_fwd(const CinShape& s, const int32_t* idx, const float* table, cons
   return DTB_OK;
 }
 
+// phase 1: dC_k (kept for every row), dZ = dC W^T and its reduction into grad_table -- after it the table gradient is
+// final; phase 2: dW_k += Z_k^T dC_k (Z_k rebuilt from the saved activations) and d_bias; phase 0: both.
 int cin_fp32_bwd(const CinShape& s, const int32_t* idx, const float* table, const int64_t* row_offsets,
                  const float* weights, const float* d_pooled, const void* saved, float* grad_table,
                  float* d_weights, float* d_bias, void* workspace, size_t workspace_bytes, int B, int act,
-                 cudaStream_t st) {
+                 int phase, cudaStream_t st) {
   (void)table;
   if (workspace_bytes < cin_fp32_workspace_bytes(s, B, 1)) {
     set_error("dtb_cin_bwd: workspace too small");
@@ -270,8 +272,8 @@ int cin_fp32_bwd(const CinShape& s, const int32_t* idx, const float* table, cons
   const int bc = fp32_chunk_rows(B, D, s.Kmax);
   float* Z = reinterpret_cast<float*>(workspace);
   float* dZ = Z + (size_t)bc * D * s.Kmax;
-  float* dC = dZ + (size_t)bc * D * s.Kmax;
-  float* dh0 = dC + (size_t)bc * D * s.Lmax;
+  float* dC_all = dZ + (size_t)bc * D * s.Kmax;
+  float* dh0 = dC_all + (size_t)B * D * s.sumL;
   float* dh1 = dh0 + (size_t)bc * D * s.Hmax;
   float* dx0t = dh1 + (size_t)bc * D * s.Hmax;
   const float* x0t_all = reinterpret_cast<const float*>(saved);
@@ -283,7 +285,15 @@ int cin_fp32_bwd(const CinShape& s, const int32_t* idx, const float* table, cons
       p += (size_t)B * D * s.L[k];
     }
   }
-  for (int b0 = 0; b0 < B; b0 += bc) {
+  float* dCk[kCinMaxLayers];
+  {
+    float* p = dC_all;
+    for (int k = 0; k < s.n_layers; ++k) {
+      dCk[k] = p;
+      p += (size_t)B * D * s.L[k];
+    }
+  }
+  for (int b0 = 0; b0 < B && phase != 2; b0 += bc) {
     const int nb = B - b0 < bc ? B - b0 : bc;
     const int64_t rows = (int64_t)nb * D;
     const float* x0t = x0t_all + (size_t)b0 * D * F;
@@ -293,25 +303,17 @@ int cin_fp32_bwd(const CinShape& s, const int32_t* idx, const float* table, cons
     for (int k = s.n_layers - 1; k >= 0; --k) {
       const int H = s.H[k], L = s.L[k], K = F * H;
       const float* T = Tk[k] + (size_t)b0 * D * L;
+      float* dC = dCk[k] + (size_t)b0 * D * L;
       const int hid_n = (k + 1 < s.n_layers) ? s.H[k + 1] : 0;
       cin_dc_kernel<<<ew_grid(rows * L), 256, 0, st>>>(T, d_pooled + (size_t)b0 * s.P, dh_next, dC, nb, D, L,
                                                        s.P, s.pool_lo[k], s.pool_n[k], s.pcol0[k], hid_n, act);
       DTB_LAUNCH_OK();
-      if (d_bias) {
-        dim3 grid(ceil_div(L, 32), 64);
-        cin_colsum_kernel<<<grid, 256, 0, st>>>(dC, d_bias + s.b_off[k], rows, L);
-        DTB_LAUNCH_OK();
-      }
       const float* hk = k == 0 ? x0t : Tk[k - 1] + (size_t)b0 * D * s.L[k - 1];
       const int ldh = k == 0 ? F : s.L[k - 1];
-      cin_build_z_kernel<<<ew_grid(rows * K), 256, 0, st>>>(x0t, hk, ldh, Z, rows, F, H);
-      DTB_LAUNCH_OK();
-      // dW_k[K, L] += Z^T dC ; dZ[rows, K] = dC W_k^T
+      // dZ[rows, K] = dC W_k^T
       {
-        int rc = dense_tc_wgrad(Z, K, dC, L, d_weights + s.w_off[k], L, nullptr, (int)rows, K, L, st);
-        if (rc == DTB_OK)
-          rc = dense_tc_rows(dC, L, weights + s.w_off[k], L, 1, nullptr, dZ, K, (int)rows, L, K, DTB_ACT_NONE, pack,
-                             pack_bytes, st);
+        const int rc = dense_tc_rows(dC, L, weights + s.w_off[k], L, 1, nullptr, dZ, K, (int)rows, L, K, DTB_ACT_NONE,
+                                     pack, pack_bytes, st);
         if (rc != DTB_OK) return rc;
       }
       int blocks = ceil_div(rows, 8);
@@ -325,6 +327,27 @@ int cin_fp32_bwd(const CinShape& s, const int32_t* idx, const float* table, cons
     cin_scatter_t_kernel<<<ew_grid((int64_t)nb * F * D), 256, 0, st>>>(idx + (size_t)b0 * F, row_offsets, dx0t,
                                                                        grad_table, nb, F, D);
     DTB_LAUNCH_OK();
+  }
+  for (int b0 = 0; b0 < B && phase != 1; b0 += bc) {
+    const int nb = B - b0 < bc ? B - b0 : bc;
+    const int64_t rows = (int64_t)nb * D;
+    const float* x0t = x0t_all + (size_t)b0 * D * F;
+    for (int k = 0; k < s.n_layers; ++k) {
+      const int H = s.H[k], L = s.L[k], K = F * H;
+      const float* dC = dCk[k] + (size_t)b0 * D * L;
+      if (d_bias) {
+        dim3 grid(ceil_div(L, 32), 64);
+        cin_colsum_kernel<<<grid, 256, 0, st>>>(dC, d_bias + s.b_off[k], rows, L);
+        DTB_LAUNCH_OK();
+      }
+      const float* hk = k == 0 ? x0t : Tk[k - 1] + (size_t)b0 * D * s.L[k - 1];
+      const int ldh = k == 0 ? F : s.L[k - 1];
+      cin_build_z_kernel<<<ew_grid(rows * K), 256, 0, st>>>(x0t, hk, ldh, Z, rows, F, H);
+      DTB_LAUNCH_OK();
+      // dW_k[K, L] += Z^T dC
+      const int rc = dense_tc_wgrad(Z, K, dC, L, d_weights + s.w_off[k], L, nullptr, (int)rows, K, L, st);
+      if (rc != DTB_OK) return rc;
+    }
   }
   return DTB_OK;
 }

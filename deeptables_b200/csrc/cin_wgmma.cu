@@ -1,0 +1,779 @@
+// CIN forward and backward fused on the Hopper tensor cores (precision codes 2-4).
+//
+// For batch row b, embedding dim d:  T_k[(b,d), l] = sum_{i,j} x0[b,i,d] h_k[b,j,d] W_k[i*H + j, l].  One warpgroup
+// owns 64 GEMM rows m = (b, d).  The A operand Z_k[m, (i,j)] = x0[m,i] h_k[m,j] never exists in memory: each thread
+// keeps h_k of its two accumulator rows in registers, in the accumulator's own fragment layout, which is also the
+// register layout wgmma expects for an A operand -- so layer k's output feeds layer k+1 without leaving the registers.
+// Per x0 field i the thread scales its h fragment by x0[m,i] and issues wgmma with A from registers; the weight chunk
+// of field i (all hidden fields x all feature maps, pre-packed as K-major bf16/fp16 core matrices) arrives in shared
+// memory by one bulk async copy, double-buffered.
+//
+// Precision: 2 = bf16x3 split (Z_hi W_hi + Z_lo W_hi + Z_hi W_lo: fp32-grade), 3 = one bf16 pass, 4 = one fp16 pass on
+// operands scaled by exact powers of two (per GEMM row for Z, per layer for W_k), undone on the fp32 accumulator.
+// The saved activations have the layout of the any-shape formulation (x0t, then T_k).  The backward (below) runs the
+// data and weight gradients as two fused wgmma kernels in bf16x3 for every precision code.
+#include "dtb_common.cuh"
+#include "cin_impl.h"
+#include "wgmma.cuh"
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+namespace dtb {
+
+constexpr int kWgRows = 64;          // GEMM rows per CTA (one m64 wgmma block)
+constexpr int kWgMaxHp = 64;         // padded hidden fields per layer (wgmma K per x0 field)
+constexpr int kWgMaxNP = 128;        // feature maps per layer (wgmma N)
+
+static inline int round_up16(int x) { return (x + 15) / 16 * 16; }
+
+struct CinWgParams {
+  const int32_t* idx;
+  const float* table;
+  const int64_t* row_offsets;
+  const uint8_t* wpack;
+  const float* bias;
+  float* pooled;
+  float* saved;          // training: x0t [B*D, F] then T_k [B*D, L_k]; null for inference
+  int* status;
+  const int* wmax;       // fp16: bit pattern of max|W_k| per layer
+  int B, D, F, n_layers, act, P;
+  int L[kCinMaxLayers], Hp[kCinMaxLayers], hid_n[kCinMaxLayers];
+  int pool_lo[kCinMaxLayers], pool_n[kCinMaxLayers], pcol0[kCinMaxLayers];
+  unsigned long long wpack_off[kCinMaxLayers], saved_off[kCinMaxLayers], bias_off[kCinMaxLayers];
+};
+
+// bytes of one x0 field's weight chunk of layer k: NP feature maps x Hp hidden fields, hi (+ lo) image
+__host__ __device__ inline uint32_t cin_wg_chunk_bytes(int NP, int Hp, int mode) {
+  return (uint32_t)NP * Hp * 2 * (mode == 0 ? 2 : 1);
+}
+
+// W_k [F*H, L] -> per field i: image of B[n][kk] = W_k[(i*H + kk), n] (zero outside H x L), core (kk/8, n/8) at
+// ((kk/8)*(NP/8) + n/8)*128 B, row n%8 at 16 B, element kk%8 at 2 B.  mode 0: bf16 hi then lo image; 1: bf16 hi only;
+// 2: fp16 of W scaled by the power of two that brings max|W_k| into [2^9, 2^10).
+__global__ void cin_wg_pack_kernel(const float* __restrict__ w, uint8_t* __restrict__ out, int F, int H, int Hp, int L,
+                                   int NP, int mode, const int* __restrict__ wmax) {
+  float s = 1.f, inv;
+  if (mode == 2) tc::pow2_scale_to_1024(__int_as_float(*wmax), s, inv);
+  const int64_t per_chunk = (int64_t)NP * Hp;
+  const int64_t total = per_chunk * F;
+  const uint32_t chunk_bytes = cin_wg_chunk_bytes(NP, Hp, mode);
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int i = (int)(t / per_chunk);
+    const int rem = (int)(t - (int64_t)i * per_chunk);
+    const int kk = rem / NP, n = rem - kk * NP;
+    const float v = (kk < H && n < L) ? w[((int64_t)i * H + kk) * L + n] : 0.f;
+    const int64_t off = ((int64_t)(kk >> 3) * (NP >> 3) + (n >> 3)) * 128 + (n & 7) * 16 + (kk & 7) * 2;
+    uint8_t* base = out + (int64_t)i * chunk_bytes;
+    if (mode == 2) {
+      *reinterpret_cast<__half*>(base + off) = __float2half_rn(v * s);
+    } else {
+      const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+      *reinterpret_cast<__nv_bfloat16*>(base + off) = hi;
+      if (mode == 0) *reinterpret_cast<__nv_bfloat16*>(base + per_chunk * 2 + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
+    }
+  }
+}
+
+__global__ void cin_wg_wmax_kernel(const float* __restrict__ w, int64_t n, int* __restrict__ out) {
+  float m = 0.f;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float a = fabsf(w[i]);
+    if (a < __int_as_float(0x7f800000)) m = fmaxf(m, a);      // ignore inf / nan
+  }
+  for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+  if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_int(m));    // non-negative floats order as ints
+}
+
+struct CinWgSmem {
+  int w_off, x0_off, out_off, bar_off, total;
+};
+__host__ __device__ inline CinWgSmem cin_wg_layout(int NP, int F, int mode) {
+  CinWgSmem l;
+  const int wbuf = (int)cin_wg_chunk_bytes(NP, kWgMaxHp, mode);
+  l.w_off = 0;
+  l.x0_off = 2 * wbuf;
+  l.out_off = l.x0_off + kWgRows * F * 4;
+  l.bar_off = (l.out_off + kWgRows * (NP + 1) * 4 + 15) / 16 * 16;
+  l.total = l.bar_off + 16;
+  return l;
+}
+
+// weight chunk number c of this CTA's schedule (tiles x layers x fields) -> source and size
+__device__ __forceinline__ void cin_wg_chunk_src(const CinWgParams& p, int NP, int mode, int k, int i, const uint8_t*& src,
+                                                 uint32_t& bytes) {
+  bytes = cin_wg_chunk_bytes(NP, p.Hp[k], mode);
+  src = p.wpack + p.wpack_off[k] + (size_t)i * bytes;
+}
+
+template <int NP, int kMode>
+__global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__ CinWgParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const CinWgSmem lay = cin_wg_layout(NP, p.F, kMode);
+  const uint32_t wbuf_bytes = cin_wg_chunk_bytes(NP, kWgMaxHp, kMode);
+  uint8_t* wbuf = smem + lay.w_off;
+  float* x0s = reinterpret_cast<float*>(smem + lay.x0_off);      // [m][i]
+  float* ot = reinterpret_cast<float*>(smem + lay.out_off);      // [m][NP + 1]
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int F = p.F, D = p.D;
+  const int64_t BD = (int64_t)p.B * D;
+  const int n_tiles = (int)((BD + kWgRows - 1) / kWgRows);
+  const int r0 = warp * 16 + (lane >> 2), c2 = 2 * (lane & 3);    // accumulator rows r0, r0 + 8; column pair base
+  constexpr uint32_t lbo_b = (NP >> 3) * 128;
+
+  if (tid == 0) {
+    tc::mbar_init(&full[0], 1);
+    tc::mbar_init(&full[1], 1);
+    tc::fence_barrier_init();
+  }
+  __syncthreads();
+  // the copy of chunk c goes to buffer c & 1; it is issued while chunk c - 1 is multiplied
+  auto issue = [&](uint32_t c, int k, int i) {
+    const uint8_t* src;
+    uint32_t bytes;
+    cin_wg_chunk_src(p, NP, kMode, k, i, src, bytes);
+    tc::mbar_arrive_expect_tx(&full[c & 1], bytes);
+    tc::bulk_g2s(wbuf + (c & 1) * wbuf_bytes, src, bytes, &full[c & 1]);
+  };
+  if (tid == 0 && (int)blockIdx.x < n_tiles) issue(0, 0, 0);
+
+  uint32_t chunk = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int64_t gm0 = (int64_t)tile * kWgRows;
+    // ---- x0 block of the 64 rows (m fastest: consecutive threads read consecutive floats of one embedding row)
+    for (int e = tid; e < kWgRows * F; e += 128) {
+      const int i = e / kWgRows, m = e - i * kWgRows;
+      const int64_t gm = gm0 + m;
+      float v = 0.f;
+      if (gm < BD) {
+        const int64_t b = gm / D;
+        const int d = (int)(gm - b * D);
+        const int64_t rb = table_row(p.row_offsets, i, __ldg(p.idx + b * F + i), D, p.status);
+        if (rb >= 0) v = __ldg(p.table + rb + d);
+        if (p.saved) p.saved[gm * F + i] = v;
+      }
+      x0s[m * F + i] = v;
+    }
+    __syncthreads();
+    // h_0 = x0, in accumulator fragment order: hh[q] = h[row r0 + 8*((q>>1)&1), col 8*(q>>2) + c2 + (q&1)]
+    float hh[kWgMaxHp / 2];
+#pragma unroll
+    for (int q = 0; q < kWgMaxHp / 2; ++q) {
+      const int row = r0 + (((q >> 1) & 1) << 3), col = 8 * (q >> 2) + c2 + (q & 1);
+      hh[q] = col < F ? x0s[row * F + col] : 0.f;
+    }
+    [[maybe_unused]] float xmax[2] = {0.f, 0.f};
+    if constexpr (kMode == 2) {
+      for (int i = 0; i < F; ++i) {
+        xmax[0] = fmaxf(xmax[0], fabsf(x0s[r0 * F + i]));
+        xmax[1] = fmaxf(xmax[1], fabsf(x0s[(r0 + 8) * F + i]));
+      }
+    }
+    for (int k = 0; k < p.n_layers; ++k) {
+      const int Hp = p.Hp[k], L = p.L[k];
+      [[maybe_unused]] float srow[2] = {1.f, 1.f}, inv_acc[2] = {1.f, 1.f};
+      if constexpr (kMode == 2) {
+        float sw, inv_w;
+        tc::pow2_scale_to_1024(__int_as_float(__ldg(p.wmax + k)), sw, inv_w);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float m = 0.f;
+#pragma unroll
+          for (int q = 0; q < kWgMaxHp / 2; ++q)
+            if (((q >> 1) & 1) == h && q < Hp / 2) m = fmaxf(m, fabsf(hh[q]));      // stale entries beyond Hp
+          m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+          m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+          float inv_row;
+          tc::pow2_scale_to_1024(xmax[h] * m, srow[h], inv_row);
+          inv_acc[h] = inv_row * inv_w;
+        }
+      }
+      float acc[NP / 2];
+#pragma unroll
+      for (int q = 0; q < NP / 2; ++q) acc[q] = 0.f;
+      for (int i = 0; i < F; ++i, ++chunk) {
+        // prefetch the next chunk of the schedule into the other buffer (its last reader finished: see the
+        // __syncthreads at the end of the previous iteration)
+        if (tid == 0) {
+          int nk = k, ni = i + 1;
+          bool more = true;
+          if (ni == F) {
+            ni = 0;
+            if (++nk == p.n_layers) { nk = 0; more = tile + (int)gridDim.x < n_tiles; }
+          }
+          if (more) issue(chunk + 1, nk, ni);
+        }
+        float x[2] = {x0s[r0 * F + i], x0s[(r0 + 8) * F + i]};
+        if constexpr (kMode == 2) { x[0] *= srow[0]; x[1] *= srow[1]; }
+        uint32_t ahi[kWgMaxHp / 16][4], alo[kWgMaxHp / 16][4];
+#pragma unroll
+        for (int ks = 0; ks < kWgMaxHp / 16; ++ks) {
+#pragma unroll
+          for (int f = 0; f < 4; ++f) {
+            const float xv = x[f & 1];
+            const float z0 = xv * hh[8 * ks + 2 * f], z1 = xv * hh[8 * ks + 2 * f + 1];
+            if constexpr (kMode == 0) tc::split_bf16x2(z0, z1, ahi[ks][f], alo[ks][f]);
+            else if constexpr (kMode == 1) ahi[ks][f] = tc::pack_bf16x2(z0, z1);
+            else ahi[ks][f] = tc::pack_f16x2(z0, z1);
+          }
+        }
+        tc::mbar_wait(&full[chunk & 1], (chunk >> 1) & 1);
+        const uint32_t b_hi = tc::smem_u32(wbuf + (chunk & 1) * wbuf_bytes);
+        const uint32_t b_lo = b_hi + (uint32_t)NP * Hp * 2;
+        tc::wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kWgMaxHp / 16; ++ks) {
+          if (ks * 16 < Hp) {
+            const uint32_t first = (i == 0 && ks == 0) ? 0u : 1u;
+            const uint64_t dh = tc::make_smem_desc(b_hi + ks * 2 * lbo_b, lbo_b, 128);
+            if constexpr (kMode == 2) {
+              tc::WgmmaF16<NP>::rs(acc, ahi[ks], dh, first);
+            } else {
+              tc::Wgmma<NP>::rs(acc, ahi[ks], dh, first);
+              if constexpr (kMode == 0) {
+                tc::Wgmma<NP>::rs(acc, alo[ks], dh, 1u);
+                tc::Wgmma<NP>::rs(acc, ahi[ks], tc::make_smem_desc(b_lo + ks * 2 * lbo_b, lbo_b, 128), 1u);
+              }
+            }
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::wgmma_fence_acc(acc);
+        __syncthreads();
+      }
+      // ---- epilogue of layer k: bias / act in registers; the tile goes through shared memory for the coalesced saved
+      //      rows and the deterministic sum over d of the pooled feature maps
+      const float* bias = p.bias ? p.bias + p.bias_off[k] : nullptr;
+      const int hid_next = k + 1 < p.n_layers ? p.hid_n[k] : 0;
+#pragma unroll
+      for (int q = 0; q < NP / 2; ++q) {
+        const int h = (q >> 1) & 1;
+        const int row = r0 + (h << 3), col = 8 * (q >> 2) + c2 + (q & 1);
+        float v = acc[q];
+        if constexpr (kMode == 2) v *= inv_acc[h];
+        if (bias && col < L) v += __ldg(bias + col);
+        if (p.act == DTB_ACT_RELU) v = fmaxf(v, 0.f);
+        if (col < L) ot[row * (NP + 1) + col] = v;
+        if (q < kWgMaxHp / 2) hh[q] = col < hid_next ? v : 0.f;
+      }
+      __syncthreads();
+      if (p.saved) {
+        float* T = p.saved + p.saved_off[k];
+        for (int e = tid; e < kWgRows * L; e += 128) {
+          const int m = e / L, col = e - m * L;
+          if (gm0 + m < BD) T[(gm0 + m) * L + col] = ot[m * (NP + 1) + col];
+        }
+      }
+      const int rows_b = kWgRows / D, pool_n = p.pool_n[k];
+      for (int e = tid; e < rows_b * pool_n; e += 128) {
+        const int bl = e / pool_n, q = e - bl * pool_n;
+        const int64_t b = gm0 / D + bl;
+        if (b < p.B) {
+          float sum = 0.f;
+          for (int d = 0; d < D; ++d) sum += ot[(bl * D + d) * (NP + 1) + p.pool_lo[k] + q];
+          p.pooled[b * p.P + p.pcol0[k] + q] = sum;
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// ==========================================================================================
+// Backward (bf16x3 split, every precision code), two kernels:
+//   dgrad, per 64-row tile, layers last -> first (one warpgroup, like the forward):
+//     dC_k = (d_pooled part + dh_{k+1}) * act'(T_k)                 registers, accumulator fragment layout
+//     dZ_{k,i}[m, j] = sum_l dC_k[m, l] W_k[i*H + j, l]             wgmma: A = dC_k from registers, B = W_k^T chunk
+//     dx0[m, i] += sum_j dZ h_k[m, j] ;  dh_k[m, j] += dZ x0[m, i]   registers (dh_k feeds dC_{k-1})
+//     dC_k is stored (fp32) for the weight gradient; dx0 is scattered into grad_table.
+//   wgrad, per (layer k, x0 field i, row split):
+//     dW_k[i*H + j, l] += sum_m x0[m, i] h_k[m, j] dC_k[m, l]       wgmma: A = x0 h from registers (rows j),
+//                                                                   B = dC_k block as a K-major image (K = m)
+// ==========================================================================================
+struct CinWgBwdParams {
+  const int32_t* idx;
+  const int64_t* row_offsets;
+  const uint8_t* wpack;      // per layer, per field: W_k^T image [NPJ x LP], hi then lo
+  const float* d_pooled;
+  const float* saved;        // x0t [B*D, F] then T_k [B*D, L_k]
+  float* grad_table;
+  float* dc;                 // dC_k [B*D, L_k] per layer
+  int B, D, F, n_layers, act, P;
+  int L[kCinMaxLayers], LP[kCinMaxLayers], H[kCinMaxLayers], hid_n[kCinMaxLayers];
+  int pool_lo[kCinMaxLayers], pool_n[kCinMaxLayers], pcol0[kCinMaxLayers];
+  unsigned long long wpack_off[kCinMaxLayers], saved_off[kCinMaxLayers], dc_off[kCinMaxLayers];
+};
+
+// W_k [F*H, L] -> per field i: K-major image of B[n][kk] = W_k[i*H + n, kk] (n < H, kk < L, else 0), N = NPJ, K = LP
+__global__ void cin_wg_pack_t_kernel(const float* __restrict__ w, uint8_t* __restrict__ out, int F, int H, int L, int LP,
+                                     int NPJ) {
+  const int64_t per_chunk = (int64_t)NPJ * LP;
+  const int64_t total = per_chunk * F;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int i = (int)(t / per_chunk);
+    const int rem = (int)(t - (int64_t)i * per_chunk);
+    const int n = rem / LP, kk = rem - n * LP;          // kk fastest: coalesced reads of W rows
+    const float v = (n < H && kk < L) ? w[((int64_t)i * H + n) * L + kk] : 0.f;
+    const int64_t off = ((int64_t)(kk >> 3) * (NPJ >> 3) + (n >> 3)) * 128 + (n & 7) * 16 + (kk & 7) * 2;
+    uint8_t* base = out + (int64_t)i * per_chunk * 4;
+    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+    *reinterpret_cast<__nv_bfloat16*>(base + off) = hi;
+    *reinterpret_cast<__nv_bfloat16*>(base + per_chunk * 2 + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
+  }
+}
+
+struct CinWgBwdSmem {
+  int w_off, x0_off, dx_off, bar_off, total;
+};
+__host__ __device__ inline CinWgBwdSmem cin_wg_bwd_layout(int NPJ, int F) {
+  CinWgBwdSmem l;
+  l.w_off = 0;
+  l.x0_off = 2 * NPJ * kWgMaxNP * 4;                 // two W^T chunk buffers (hi + lo)
+  l.dx_off = l.x0_off + kWgRows * F * 4;
+  l.bar_off = (l.dx_off + kWgRows * F * 4 + 15) / 16 * 16;
+  l.total = l.bar_off + 16;
+  return l;
+}
+
+template <int NPJ>
+__global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant__ CinWgBwdParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const CinWgBwdSmem lay = cin_wg_bwd_layout(NPJ, p.F);
+  constexpr uint32_t wbuf_bytes = NPJ * kWgMaxNP * 4;
+  uint8_t* wbuf = smem + lay.w_off;
+  float* x0s = reinterpret_cast<float*>(smem + lay.x0_off);      // [m][i]
+  float* dxs = reinterpret_cast<float*>(smem + lay.dx_off);      // [m][i]
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int F = p.F, D = p.D;
+  const int64_t BD = (int64_t)p.B * D;
+  const int n_tiles = (int)((BD + kWgRows - 1) / kWgRows);
+  const int r0 = warp * 16 + (lane >> 2), c2 = 2 * (lane & 3);
+  constexpr uint32_t lbo_b = (NPJ >> 3) * 128;
+  const int K0 = p.n_layers - 1;
+
+  if (tid == 0) {
+    tc::mbar_init(&full[0], 1);
+    tc::mbar_init(&full[1], 1);
+    tc::fence_barrier_init();
+  }
+  __syncthreads();
+  auto issue = [&](uint32_t c, int k, int i) {
+    const uint32_t bytes = (uint32_t)NPJ * p.LP[k] * 4;
+    tc::mbar_arrive_expect_tx(&full[c & 1], bytes);
+    tc::bulk_g2s(wbuf + (c & 1) * wbuf_bytes, p.wpack + p.wpack_off[k] + (size_t)i * bytes, bytes, &full[c & 1]);
+  };
+  if (tid == 0 && (int)blockIdx.x < n_tiles) issue(0, K0, 0);
+
+  uint32_t chunk = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int64_t gm0 = (int64_t)tile * kWgRows;
+    for (int e = tid; e < kWgRows * F; e += 128) {
+      const int m = e / F;
+      x0s[e] = gm0 + m < BD ? p.saved[gm0 * F + e] : 0.f;
+      dxs[e] = 0.f;
+    }
+    __syncthreads();
+    float dh[NPJ / 2];                   // gradient wrt h_{k+1}, accumulator fragment order (columns j)
+#pragma unroll
+    for (int q = 0; q < NPJ / 2; ++q) dh[q] = 0.f;
+    for (int k = K0; k >= 0; --k) {
+      const int L = p.L[k], LP = p.LP[k], H = p.H[k];
+      // ---- dC_k in A-fragment order: dc element q <-> row r0 + 8*((q>>1)&1), column l = 8*(q>>2) + c2 + (q&1)
+      uint32_t ahi[kWgMaxNP / 16][4], alo[kWgMaxNP / 16][4];
+      {
+        const float* T = p.saved + p.saved_off[k];
+        float* dcg = p.dc + p.dc_off[k];
+#pragma unroll
+        for (int q = 0; q < kWgMaxNP / 2; q += 2) {
+          const int row = r0 + (((q >> 1) & 1) << 3), l = 8 * (q >> 2) + c2;
+          const int64_t gm = gm0 + row;
+          float g[2] = {0.f, 0.f};
+          if (gm < BD && l < LP) {
+            const int64_t b = gm / D;
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const int lu = l + u;
+              if (lu < L) {
+                if (lu >= p.pool_lo[k] && lu < p.pool_lo[k] + p.pool_n[k])
+                  g[u] += __ldg(p.d_pooled + b * p.P + p.pcol0[k] + lu - p.pool_lo[k]);
+                if (lu < p.hid_n[k] && q + u < NPJ / 2) g[u] += dh[q + u];
+                if (p.act == DTB_ACT_RELU && !(T[gm * L + lu] > 0.f)) g[u] = 0.f;
+                dcg[gm * L + lu] = g[u];
+              }
+            }
+          }
+          tc::split_bf16x2(g[0], g[1], ahi[q >> 3][(q >> 1) & 3], alo[q >> 3][(q >> 1) & 3]);
+        }
+      }
+      // h_k in fragment order (columns j), and the fresh dh_k accumulators
+      float hh[NPJ / 2];
+      {
+        const float* hsrc = k == 0 ? nullptr : p.saved + p.saved_off[k - 1];
+        const int ldh = k == 0 ? F : p.L[k - 1];
+#pragma unroll
+        for (int q = 0; q < NPJ / 2; ++q) {
+          const int row = r0 + (((q >> 1) & 1) << 3), j = 8 * (q >> 2) + c2 + (q & 1);
+          const int64_t gm = gm0 + row;
+          hh[q] = (j < H && gm < BD) ? (k == 0 ? x0s[row * F + j] : hsrc[gm * ldh + j]) : 0.f;
+          dh[q] = 0.f;
+        }
+      }
+      for (int i = 0; i < F; ++i, ++chunk) {
+        if (tid == 0) {
+          int nk = k, ni = i + 1;
+          bool more = true;
+          if (ni == F) {
+            ni = 0;
+            if (--nk < 0) { nk = K0; more = tile + (int)gridDim.x < n_tiles; }
+          }
+          if (more) issue(chunk + 1, nk, ni);
+        }
+        float acc[NPJ / 2];
+#pragma unroll
+        for (int q = 0; q < NPJ / 2; ++q) acc[q] = 0.f;
+        tc::mbar_wait(&full[chunk & 1], (chunk >> 1) & 1);
+        const uint32_t b_hi = tc::smem_u32(wbuf + (chunk & 1) * wbuf_bytes);
+        const uint32_t b_lo = b_hi + (uint32_t)NPJ * LP * 2;
+        tc::wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kWgMaxNP / 16; ++ks) {
+          if (ks * 16 < LP) {
+            const uint64_t dh_desc = tc::make_smem_desc(b_hi + ks * 2 * lbo_b, lbo_b, 128);
+            tc::Wgmma<NPJ>::rs(acc, ahi[ks], dh_desc, ks == 0 ? 0u : 1u);
+            tc::Wgmma<NPJ>::rs(acc, alo[ks], dh_desc, 1u);
+            tc::Wgmma<NPJ>::rs(acc, ahi[ks], tc::make_smem_desc(b_lo + ks * 2 * lbo_b, lbo_b, 128), 1u);
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::wgmma_fence_acc(acc);
+        // dx0[m, i] += sum_j dZ h ; dh[m, j] += dZ x0[m, i]
+        const float x_a = x0s[r0 * F + i], x_b = x0s[(r0 + 8) * F + i];
+        float s_a = 0.f, s_b = 0.f;
+#pragma unroll
+        for (int q = 0; q < NPJ / 2; ++q) {
+          if ((q >> 1) & 1) { s_b += acc[q] * hh[q]; dh[q] += acc[q] * x_b; }
+          else              { s_a += acc[q] * hh[q]; dh[q] += acc[q] * x_a; }
+        }
+        s_a += __shfl_xor_sync(0xffffffffu, s_a, 1);
+        s_a += __shfl_xor_sync(0xffffffffu, s_a, 2);
+        s_b += __shfl_xor_sync(0xffffffffu, s_b, 1);
+        s_b += __shfl_xor_sync(0xffffffffu, s_b, 2);
+        if ((lane & 3) == 0) {
+          dxs[r0 * F + i] += s_a;
+          dxs[(r0 + 8) * F + i] += s_b;
+        }
+        __syncthreads();
+      }
+    }
+    // layer 0: h_0 is x0 itself, so dh_0 adds to dx0; then scatter into the table gradient
+#pragma unroll
+    for (int q = 0; q < NPJ / 2; ++q) {
+      const int row = r0 + (((q >> 1) & 1) << 3), j = 8 * (q >> 2) + c2 + (q & 1);
+      if (j < F) dxs[row * F + j] += dh[q];
+    }
+    __syncthreads();
+    for (int e = tid; e < kWgRows * F; e += 128) {
+      const int i = e / kWgRows, m = e - i * kWgRows;
+      const int64_t gm = gm0 + m;
+      if (gm < BD) {
+        const int64_t b = gm / D;
+        const int64_t rb = table_row(p.row_offsets, i, __ldg(p.idx + b * F + i), D, nullptr);
+        if (rb >= 0) atomicAdd(p.grad_table + rb + (gm - b * D), dxs[m * F + i]);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+struct CinWgWgradParams {
+  const float* x0t;      // [B*D, F]
+  const float* h;        // h_k rows: x0t (k = 0) or T_{k-1}, leading dimension ldh
+  const float* dc;       // dC_k [B*D, L]
+  float* dw;             // dW_k [F*H, L]
+  float* dbias;          // [L] or null
+  int64_t BD;
+  int F, H, L, ldh, blocks_per_split;
+};
+
+template <int NP>
+__global__ void __launch_bounds__(128) cin_wg_wgrad_kernel(const __grid_constant__ CinWgWgradParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint8_t* bimg = smem;                                                          // dC block, K-major (K = m), hi | lo
+  float (*hs)[kWgMaxHp + 1] = reinterpret_cast<float (*)[kWgMaxHp + 1]>(smem + 2 * NP * kWgRows * 2);
+  float* xs = reinterpret_cast<float*>(smem + 2 * NP * kWgRows * 2 + kWgRows * (kWgMaxHp + 1) * 4);
+  float* bsum = xs + kWgRows;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int i = blockIdx.x;
+  const int j0 = warp * 16 + (lane >> 2), c2 = 2 * (lane & 3);           // A rows j0, j0 + 8; k columns m
+  constexpr uint32_t lbo_b = (NP >> 3) * 128;
+  constexpr uint32_t img = NP * kWgRows * 2;
+  const bool do_bias = p.dbias && i == 0;
+  for (int l = tid; l < NP; l += 128) bsum[l] = 0.f;
+  float acc[NP / 2];
+#pragma unroll
+  for (int q = 0; q < NP / 2; ++q) acc[q] = 0.f;
+  const int64_t n_blocks = (p.BD + kWgRows - 1) / kWgRows;
+  const int64_t blk0 = (int64_t)blockIdx.y * p.blocks_per_split;
+  int64_t blk1 = blk0 + p.blocks_per_split;
+  if (blk1 > n_blocks) blk1 = n_blocks;
+  for (int64_t blk = blk0; blk < blk1; ++blk) {
+    const int64_t gm0 = blk * kWgRows;
+    __syncthreads();                                       // the previous block's MMAs and reads are done
+    for (int e = tid; e < kWgRows * p.H; e += 128) {
+      const int m = e / p.H, j = e - m * p.H;
+      hs[m][j] = gm0 + m < p.BD ? p.h[(gm0 + m) * p.ldh + j] : 0.f;
+    }
+    if (tid < kWgRows) xs[tid] = gm0 + tid < p.BD ? p.x0t[(gm0 + tid) * p.F + i] : 0.f;
+    for (int e = tid; e < kWgRows * NP; e += 128) {
+      const int m = e / NP, l = e - m * NP;
+      const float v = (gm0 + m < p.BD && l < p.L) ? p.dc[(gm0 + m) * p.L + l] : 0.f;
+      if (do_bias && v != 0.f) atomicAdd(&bsum[l], v);
+      const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+      const int off = ((m >> 3) * (NP >> 3) + (l >> 3)) * 128 + (l & 7) * 16 + (m & 7) * 2;
+      *reinterpret_cast<__nv_bfloat16*>(bimg + off) = hi;
+      *reinterpret_cast<__nv_bfloat16*>(bimg + img + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
+    }
+    tc::fence_proxy_async_smem();
+    __syncthreads();
+    const uint32_t b_hi = tc::smem_u32(bimg), b_lo = b_hi + img;
+    uint32_t ahi[kWgRows / 16][4], alo[kWgRows / 16][4];
+#pragma unroll
+    for (int ks = 0; ks < kWgRows / 16; ++ks) {
+#pragma unroll
+      for (int f = 0; f < 4; ++f) {
+        const int j = j0 + ((f & 1) << 3), m = ks * 16 + ((f >> 1) << 3) + c2;
+        const float z0 = j < p.H ? xs[m] * hs[m][j] : 0.f, z1 = j < p.H ? xs[m + 1] * hs[m + 1][j] : 0.f;
+        tc::split_bf16x2(z0, z1, ahi[ks][f], alo[ks][f]);
+      }
+    }
+    tc::wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kWgRows / 16; ++ks) {
+      const uint64_t dhi = tc::make_smem_desc(b_hi + ks * 2 * lbo_b, lbo_b, 128);
+      tc::Wgmma<NP>::rs(acc, ahi[ks], dhi, 1u);
+      tc::Wgmma<NP>::rs(acc, alo[ks], dhi, 1u);
+      tc::Wgmma<NP>::rs(acc, ahi[ks], tc::make_smem_desc(b_lo + ks * 2 * lbo_b, lbo_b, 128), 1u);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::wgmma_fence_acc(acc);
+  }
+#pragma unroll
+  for (int q = 0; q < NP / 2; ++q) {
+    const int j = j0 + (((q >> 1) & 1) << 3), l = 8 * (q >> 2) + c2 + (q & 1);
+    if (j < p.H && l < p.L && acc[q] != 0.f) atomicAdd(p.dw + ((int64_t)i * p.H + j) * p.L + l, acc[q]);
+  }
+  if (do_bias) {
+    __syncthreads();
+    for (int l = tid; l < p.L; l += 128)
+      if (bsum[l] != 0.f) atomicAdd(p.dbias + l, bsum[l]);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// host side
+// ------------------------------------------------------------------------------------------
+static int cin_wg_np(const CinShape& s) {
+  int np = 16;
+  while (np < s.Lmax) np *= 2;
+  return np;
+}
+
+bool cin_wg_supported(const CinShape& s) {
+  if (!(s.D == 4 || s.D == 8 || s.D == 16 || s.D == 32)) return false;      // D divides the 64-row tile
+  if (s.F < 1 || s.F > kWgMaxHp || s.Lmax > kWgMaxNP) return false;
+  for (int k = 0; k < s.n_layers; ++k)
+    if (round_up16(s.H[k]) > kWgMaxHp) return false;
+  return cin_wg_layout(cin_wg_np(s), s.F, 0).total <= 227 * 1024;
+}
+
+size_t cin_wg_workspace_bytes(const CinShape& s) {
+  const int np = cin_wg_np(s);
+  size_t b = 0;
+  for (int k = 0; k < s.n_layers; ++k) b += (size_t)s.F * cin_wg_chunk_bytes(np, round_up16(s.H[k]), 0);
+  return b + 256;      // + the max|W_k| words of the fp16 variant
+}
+
+template <int NP, int kMode>
+static int cin_wg_launch(const CinWgParams& p, cudaStream_t st) {
+  const CinWgSmem lay = cin_wg_layout(NP, p.F, kMode);
+  DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_fwd_kernel<NP, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+  const int64_t n_tiles = ((int64_t)p.B * p.D + kWgRows - 1) / kWgRows;
+  int per_sm = (227 * 1024) / (lay.total + 1024);
+  if (per_sm < 1) per_sm = 1;
+  if (per_sm > 4) per_sm = 4;
+  int64_t grid = (int64_t)sm_count() * per_sm;
+  if (grid > n_tiles) grid = n_tiles;
+  cin_wg_fwd_kernel<NP, kMode><<<(int)grid, 128, lay.total, st>>>(p);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
+
+template <int kMode>
+static int cin_wg_dispatch(const CinWgParams& p, int np, cudaStream_t st) {
+  switch (np) {
+    case 16: return cin_wg_launch<16, kMode>(p, st);
+    case 32: return cin_wg_launch<32, kMode>(p, st);
+    case 64: return cin_wg_launch<64, kMode>(p, st);
+    default: return cin_wg_launch<128, kMode>(p, st);
+  }
+}
+
+int cin_wg_fwd(const CinShape& s, const int32_t* idx, const float* table, const int64_t* row_offsets,
+               const float* weights, const float* bias, float* pooled, void* saved, void* workspace,
+               size_t workspace_bytes, int B, int act, int mode, int* status, cudaStream_t st) {
+  if (workspace_bytes < cin_wg_workspace_bytes(s) || (reinterpret_cast<uintptr_t>(workspace) & 127)) {
+    set_error("dtb_cin_fwd: workspace too small or not 128-byte aligned for the packed weights");
+    return DTB_ERR_INVALID_ARG;
+  }
+  const int np = cin_wg_np(s);
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  int* wmax = reinterpret_cast<int*>(ws + cin_wg_workspace_bytes(s) - 256);
+  CinWgParams p{};
+  p.idx = idx; p.table = table; p.row_offsets = row_offsets; p.wpack = ws; p.bias = bias; p.pooled = pooled;
+  p.saved = reinterpret_cast<float*>(saved); p.status = status; p.wmax = wmax;
+  p.B = B; p.D = s.D; p.F = s.F; p.n_layers = s.n_layers; p.act = act; p.P = s.P;
+  if (mode == 2) DTB_CUDA_OK(cudaMemsetAsync(wmax, 0, sizeof(int) * kCinMaxLayers, st));
+  size_t woff = 0, soff = (size_t)B * s.D * s.F;
+  for (int k = 0; k < s.n_layers; ++k) {
+    p.L[k] = s.L[k]; p.Hp[k] = round_up16(s.H[k]); p.hid_n[k] = k + 1 < s.n_layers ? s.H[k + 1] : 0;
+    p.pool_lo[k] = s.pool_lo[k]; p.pool_n[k] = s.pool_n[k]; p.pcol0[k] = s.pcol0[k];
+    p.wpack_off[k] = woff; p.saved_off[k] = soff; p.bias_off[k] = s.b_off[k];
+    const int64_t n_w = (int64_t)s.F * s.H[k] * s.L[k];
+    if (mode == 2) {
+      cin_wg_wmax_kernel<<<(int)((n_w + 255) / 256 < 64 ? (n_w + 255) / 256 : 64), 256, 0, st>>>(weights + s.w_off[k], n_w,
+                                                                                                 wmax + k);
+      DTB_LAUNCH_OK();
+    }
+    const int64_t total = (int64_t)s.F * np * p.Hp[k];
+    int blocks = (int)((total + 255) / 256);
+    if (blocks > sm_count() * 8) blocks = sm_count() * 8;
+    cin_wg_pack_kernel<<<blocks, 256, 0, st>>>(weights + s.w_off[k], ws + woff, s.F, s.H[k], p.Hp[k], s.L[k], np, mode,
+                                               wmax + k);
+    DTB_LAUNCH_OK();
+    woff += (size_t)s.F * cin_wg_chunk_bytes(np, p.Hp[k], mode);
+    soff += (size_t)B * s.D * s.L[k];
+  }
+  switch (mode) {
+    case 0: return cin_wg_dispatch<0>(p, np, st);
+    case 1: return cin_wg_dispatch<1>(p, np, st);
+    default: return cin_wg_dispatch<2>(p, np, st);
+  }
+}
+
+static int cin_wg_npj(const CinShape& s) {
+  int hp = 16;
+  for (int k = 0; k < s.n_layers; ++k) hp = round_up16(s.H[k]) > hp ? round_up16(s.H[k]) : hp;
+  int np = 16;
+  while (np < hp) np *= 2;
+  return np;
+}
+static size_t cin_wg_pack_t_bytes(const CinShape& s) {
+  size_t b = 0;
+  for (int k = 0; k < s.n_layers; ++k) b += (size_t)s.F * cin_wg_npj(s) * round_up16(s.L[k]) * 4;
+  return (b + 255) / 256 * 256;
+}
+size_t cin_wg_bwd_workspace_bytes(const CinShape& s, int B) {
+  return cin_wg_pack_t_bytes(s) + (size_t)B * s.D * s.sumL * sizeof(float);
+}
+static int wgrad_smem_bytes(int NP) { return 2 * NP * kWgRows * 2 + kWgRows * (kWgMaxHp + 1) * 4 + kWgRows * 4 + NP * 4; }
+
+template <int NPJ>
+static int cin_wg_dgrad_launch(const CinWgBwdParams& p, cudaStream_t st) {
+  const CinWgBwdSmem lay = cin_wg_bwd_layout(NPJ, p.F);
+  DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_dgrad_kernel<NPJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+  const int64_t n_tiles = ((int64_t)p.B * p.D + kWgRows - 1) / kWgRows;
+  int per_sm = (227 * 1024) / (lay.total + 1024);
+  per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
+  int64_t grid = (int64_t)sm_count() * per_sm;
+  if (grid > n_tiles) grid = n_tiles;
+  cin_wg_dgrad_kernel<NPJ><<<(int)grid, 128, lay.total, st>>>(p);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
+
+template <int NP>
+static int cin_wg_wgrad_launch(const CinWgWgradParams& p, int n_splits, cudaStream_t st) {
+  const int smem = wgrad_smem_bytes(NP);
+  DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_wgrad_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  cin_wg_wgrad_kernel<NP><<<dim3(p.F, n_splits), 128, smem, st>>>(p);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
+
+int cin_wg_bwd(const CinShape& s, const int32_t* idx, const int64_t* row_offsets, const float* weights,
+               const float* d_pooled, const void* saved, float* grad_table, float* d_weights, float* d_bias,
+               void* workspace, size_t workspace_bytes, int B, int act, int phase, cudaStream_t st) {
+  if (workspace_bytes < cin_wg_bwd_workspace_bytes(s, B) || (reinterpret_cast<uintptr_t>(workspace) & 127)) {
+    set_error("dtb_cin_bwd: workspace too small or not 128-byte aligned");
+    return DTB_ERR_INVALID_ARG;
+  }
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  float* dc = reinterpret_cast<float*>(ws + cin_wg_pack_t_bytes(s));
+  const float* sv = reinterpret_cast<const float*>(saved);
+  const int npj = cin_wg_npj(s);
+  size_t dc_off[kCinMaxLayers], saved_off[kCinMaxLayers];
+  {
+    size_t d = 0, o = (size_t)B * s.D * s.F;
+    for (int k = 0; k < s.n_layers; ++k) {
+      dc_off[k] = d; saved_off[k] = o;
+      d += (size_t)B * s.D * s.L[k];
+      o += (size_t)B * s.D * s.L[k];
+    }
+  }
+  if (phase != 2) {
+    CinWgBwdParams p{};
+    p.idx = idx; p.row_offsets = row_offsets; p.wpack = ws; p.d_pooled = d_pooled; p.saved = sv;
+    p.grad_table = grad_table; p.dc = dc;
+    p.B = B; p.D = s.D; p.F = s.F; p.n_layers = s.n_layers; p.act = act; p.P = s.P;
+    size_t woff = 0;
+    for (int k = 0; k < s.n_layers; ++k) {
+      p.L[k] = s.L[k]; p.LP[k] = round_up16(s.L[k]); p.H[k] = s.H[k]; p.hid_n[k] = k + 1 < s.n_layers ? s.H[k + 1] : 0;
+      p.pool_lo[k] = s.pool_lo[k]; p.pool_n[k] = s.pool_n[k]; p.pcol0[k] = s.pcol0[k];
+      p.wpack_off[k] = woff; p.saved_off[k] = saved_off[k]; p.dc_off[k] = dc_off[k];
+      const int64_t total = (int64_t)s.F * npj * p.LP[k];
+      int blocks = (int)((total + 255) / 256);
+      if (blocks > sm_count() * 8) blocks = sm_count() * 8;
+      cin_wg_pack_t_kernel<<<blocks, 256, 0, st>>>(weights + s.w_off[k], ws + woff, s.F, s.H[k], s.L[k], p.LP[k], npj);
+      DTB_LAUNCH_OK();
+      woff += (size_t)s.F * npj * p.LP[k] * 4;
+    }
+    int rc;
+    switch (npj) {
+      case 16: rc = cin_wg_dgrad_launch<16>(p, st); break;
+      case 32: rc = cin_wg_dgrad_launch<32>(p, st); break;
+      default: rc = cin_wg_dgrad_launch<64>(p, st); break;
+    }
+    if (rc != DTB_OK) return rc;
+  }
+  if (phase != 1) {
+    const int np = cin_wg_np(s);
+    const int64_t BD = (int64_t)B * s.D;
+    const int64_t n_blocks = (BD + kWgRows - 1) / kWgRows;
+    for (int k = 0; k < s.n_layers; ++k) {
+      CinWgWgradParams w{};
+      w.x0t = sv; w.h = k == 0 ? sv : sv + saved_off[k - 1]; w.ldh = k == 0 ? s.F : s.L[k - 1];
+      w.dc = dc + dc_off[k]; w.dw = d_weights + s.w_off[k]; w.dbias = d_bias ? d_bias + s.b_off[k] : nullptr;
+      w.BD = BD; w.F = s.F; w.H = s.H[k]; w.L = s.L[k];
+      int64_t splits = (int64_t)sm_count() * 2 / s.F;
+      if (splits < 1) splits = 1;
+      if (splits > n_blocks) splits = n_blocks;
+      w.blocks_per_split = (int)((n_blocks + splits - 1) / splits);
+      splits = (n_blocks + w.blocks_per_split - 1) / w.blocks_per_split;
+      int rc;
+      switch (np) {
+        case 16: rc = cin_wg_wgrad_launch<16>(w, (int)splits, st); break;
+        case 32: rc = cin_wg_wgrad_launch<32>(w, (int)splits, st); break;
+        case 64: rc = cin_wg_wgrad_launch<64>(w, (int)splits, st); break;
+        default: rc = cin_wg_wgrad_launch<128>(w, (int)splits, st); break;
+      }
+      if (rc != DTB_OK) return rc;
+    }
+  }
+  return DTB_OK;
+}
+
+}  // namespace dtb

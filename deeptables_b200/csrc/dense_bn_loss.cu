@@ -512,7 +512,7 @@ int dtb_dense_fwd(const float* X, const float* W, const float* bias, float* Y, v
     DTB_LAUNCH_OK();
     return DTB_OK;
   }
-  // tcgen05 GEMM with the bias / activation epilogue fused (dense_tc.cu)
+  // wgmma GEMM with the bias / activation epilogue fused (dense_tc.cu)
   return dense_tc_rows(X, in_dim, W, out_dim, 0, bias, Y, out_dim, rows, in_dim, out_dim, act, workspace,
                        workspace_bytes, st);
 }
@@ -549,7 +549,7 @@ int dtb_dense_bwd(const float* X, const float* W, const float* Y, float* dY, flo
     }
     return DTB_OK;
   }
-  // dW[in,out] += X^T dZ and dbias += colsum(dZ) in one tcgen05 kernel; dX[rows,in] = dZ W^T in another
+  // dW[in,out] += X^T dZ and dbias += colsum(dZ) in one wgmma kernel; dX[rows,in] = dZ W^T in another
   int rc = dense_tc_wgrad(X, in_dim, dY, out_dim, dW, out_dim, dbias, rows, in_dim, out_dim, st);
   if (rc != DTB_OK) return rc;
   if (dX)

@@ -1,9 +1,9 @@
-// Dense-layer GEMMs on the 5th-generation tensor cores (tcgen05 + TMEM): keras Dense forward / data gradient /
+// Dense-layer GEMMs on the Hopper tensor cores (wgmma, fp32 accumulators in registers): keras Dense forward / data gradient /
 // weight gradient (dnn() tower, deepnets.py:401-427; per-net logit layers wider than 8, deepmodel.py:292; the AutoInt
 // Q/K/V/residual projections, layers.py:106-127) and the GEMMs of the any-shape CIN formulation (cin_fp32.cu).
 //
 // fp32 in, fp32 out.  Operands are split on the fly into bf16 hi + lo and multiplied in three tensor passes
-// (hi*hi + lo*hi + hi*lo, fp32 accumulation in TMEM): each operand is represented to 2^-18, the dropped lo*lo term is
+// (hi*hi + lo*hi + hi*lo, fp32 accumulation): each operand is represented to 2^-18, the dropped lo*lo term is
 // 2^-18 of a product, i.e. fp32-grade results (the same scheme the CIN kernels use, cin_tc.cu).
 //
 //   rows kernel   out[M, Nout] = act(A[M, K] . W + bias)       W given as packed images (dense_tc_pack_kernel)
@@ -12,27 +12,26 @@
 //   wgrad kernel  dW[K, N] += sum_m X[m, k] dZ[m, n]     both operands converted on the fly; reduction over batch rows
 //
 // These shapes are HBM-bound (126 kFLOP per 1.7 KB row for 429 -> 128 -> 64), so the structure is a streaming one:
-// coalesced fp32 reads -> registers -> bf16 hi/lo core matrices in shared memory (UMMA canonical K-major, no swizzle)
-// -> tcgen05.mma (SS form), 4-stage mbarrier ring, weights by bulk async copy, double-buffered TMEM accumulators whose
-// read-out (bias / relu; lane = output row, 32 columns per TMEM read written as 8 float4 of the lane's own 128-byte line)
-// overlaps the next tile's loads.  Outputs whose rows are not 16-byte aligned go through a shared-memory transpose instead
-// (also selectable with DTB_DENSE_DIRECT=0: it was the only form until the [B*F, 32] -> 128 AutoInt projection measured
-// 0.82 ms against 0.44 ms for the direct stores).
+// coalesced fp32 reads -> registers -> bf16 hi/lo core matrices in shared memory (canonical K-major, no swizzle)
+// -> wgmma (both operands from shared memory), 4-stage mbarrier ring, weights by bulk async copy.  Two consumer
+// warpgroups own 64 rows each of a 128-row tile; they release a stage as soon as their MMAs on it complete, so the
+// producers and the weight loader run up to four stages ahead while the consumers apply bias / activation to their
+// accumulator registers and store them.
 #include "dtb_common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include "dense_tc.h"
 #include <cuda_bf16.h>
 #include <cstdlib>
 
 namespace dtb {
 
-constexpr int kDtThreads = 448;        // rows kernel: warps 0-7 producers, 8-11 epilogue, 12 MMA issue + TMEM owner, 13 weight loader
-constexpr int kDtWgThreads = 320;      // wgrad kernel: warps 0-3 X producers (+ epilogue), 4-7 dZ producers, 8 MMA issue
-constexpr int kDtKc = 32;              // reduction elements per pipeline stage (two UMMA k-steps)
+constexpr int kDtThreads = 544;        // rows kernel: warps 0-7 producers, 8-15 two MMA + epilogue warpgroups, 16 weight loader
+constexpr int kDtWgThreads = 512;      // wgrad kernel: warps 0-3 X producers, 4-7 dZ producers, 8-15 two MMA + epilogue warpgroups
+constexpr int kDtKc = 32;              // reduction elements per pipeline stage (two wgmma k-steps)
 constexpr int kDtStages = 4;
 constexpr int kDtAImg = 128 * kDtKc * 2;          // bytes of one bf16 [128 x 32] image
 constexpr int kDtAStage = 2 * kDtAImg;            // hi + lo
-constexpr int kDtMaxNT = 256;
+constexpr int kDtMaxNT = 128;            // widest wgmma N used (64 accumulator registers per thread)
 
 static inline int dt_round_up(int x, int m) { return (x + m - 1) / m * m; }
 
@@ -70,38 +69,25 @@ struct DenseTcRowsParams {
   const uint8_t* wpack;  // images [n_tile][k_chunk][hi | lo]
   const float* bias;     // [Nout] or null
   float* out;            // [M, Nout], leading dimension ldo
-  int M, K, Nout, lda, ldo, NT, n_tiles, n_chunks, act, direct;
+  int M, K, Nout, lda, ldo, NT, n_tiles, n_chunks, act, vec2;
 };
 
 struct DtSmem {
-  int a_off, b_off, t_off, bar_off, total, b_stage;
+  int a_off, b_off, bar_off, total, b_stage;
 };
-__host__ __device__ inline DtSmem dt_layout(int NT, int with_tbuf) {
+__host__ __device__ inline DtSmem dt_layout(int NT) {
   DtSmem l;
   l.b_stage = NT * kDtKc * 4;
   l.a_off = 0;
   l.b_off = kDtStages * kDtAStage;
-  l.t_off = l.b_off + kDtStages * l.b_stage;
-  l.bar_off = l.t_off + (with_tbuf ? 4 * 32 * 17 * 4 : 0);
+  l.bar_off = l.b_off + kDtStages * l.b_stage;
   l.bar_off = (l.bar_off + 15) / 16 * 16;
   l.total = l.bar_off + 256;
   return l;
 }
 
-__device__ __forceinline__ bool dt_elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // [16 rows x 32 columns] fp32 block of a row-major matrix -> registers (one 128-byte request per row, all 16 in flight),
-// and registers -> bf16 hi/lo words of a K-major image whose UMMA rows are the matrix ROWS and whose reduction index is
+// and registers -> bf16 hi/lo words of a K-major image whose MMA rows are the matrix ROWS and whose reduction index is
 // the matrix COLUMN (rows kernel: A = X tile).  A lane pair (k even, k+1) exchanges values so that the even lane stores
 // the packed hi word and the odd lane the packed lo word.
 __device__ __forceinline__ void dt_load_rows16(float (&v)[16], const float* __restrict__ src, int ld, int row0,
@@ -127,19 +113,40 @@ __device__ __forceinline__ void dt_store_rows16(const float (&v)[16], uint8_t* i
   }
 }
 
+// One k-chunk (kDtKc = 32) of the three bf16 passes on this warpgroup's 64 rows: A image rows [64 wg, 64 wg + 64),
+// B image NT rows; then wait for the MMAs, so that the caller may release the stage.
+template <int NT>
+__device__ __forceinline__ void dt_mma_chunk(float (&acc)[NT / 2], uint32_t a_addr, uint32_t b_addr, int wg, bool first) {
+  constexpr uint32_t lbo_b = (NT >> 3) * 128;
+  constexpr uint32_t img_b = NT * kDtKc * 2;
+  tc::wgmma_fence();
+#pragma unroll
+  for (int pass = 0; pass < 3; ++pass) {
+    // pass 0: A_hi*B_hi ; 1: A_lo*B_hi ; 2: A_hi*B_lo
+    const uint32_t a_img = a_addr + (pass == 1 ? kDtAImg : 0) + wg * 1024;
+    const uint32_t b_img = b_addr + (pass == 2 ? img_b : 0);
+#pragma unroll
+    for (int ks = 0; ks < kDtKc / 16; ++ks) {
+      const uint64_t da = tc::make_smem_desc(a_img + ks * 4096, 2048, 128);
+      const uint64_t db = tc::make_smem_desc(b_img + ks * 2 * lbo_b, lbo_b, 128);
+      tc::Wgmma<NT>::ss(acc, da, db, (uint32_t)(!first || pass != 0 || ks != 0));
+    }
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::wgmma_fence_acc(acc);
+}
+
+template <int NT>
 __global__ void __launch_bounds__(kDtThreads, 1) dense_tc_rows_kernel(const __grid_constant__ DenseTcRowsParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const DtSmem lay = dt_layout(p.NT, 1);
+  const DtSmem lay = dt_layout(NT);
   uint8_t* smem_a = smem + lay.a_off;
   uint8_t* smem_b = smem + lay.b_off;
-  float* tbuf = reinterpret_cast<float*>(smem + lay.t_off);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
   uint64_t* full_a = bars;                 // [stage] 8 producer warps
   uint64_t* full_b = bars + 4;             // [stage] bulk copy (tx)
-  uint64_t* empty = bars + 8;              // [stage] tcgen05.commit
-  uint64_t* acc_full = bars + 12;          // [buf]   commit
-  uint64_t* acc_empty = bars + 14;         // [buf]   4 epilogue warps
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
+  uint64_t* empty = bars + 8;              // [stage] 8 consumer warps
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_mtiles = (p.M + 127) / 128;
@@ -149,25 +156,16 @@ __global__ void __launch_bounds__(kDtThreads, 1) dense_tc_rows_kernel(const __gr
     for (int s = 0; s < kDtStages; ++s) {
       tc::mbar_init(&full_a[s], 8);
       tc::mbar_init(&full_b[s], 1);
-      tc::mbar_init(&empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      tc::mbar_init(&acc_full[b], 1);
-      tc::mbar_init(&acc_empty[b], 4);
+      tc::mbar_init(&empty[s], 8);
     }
     tc::fence_barrier_init();
   }
-  if (warp == 12) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_thread_sync();
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 8) {
     // ============================ A producers: fp32 rows -> bf16 hi/lo images =============================
     // warp w converts rows [16w, 16w + 16) of the tile.  The loads of the NEXT (item, chunk) are issued before this
-    // chunk's barrier wait and conversion: 8 warps x 16-32 requests of 128 bytes keep 16-32 KB in flight per SM
-    // (the first version had 4 warps x 8: a third of the latency-bandwidth product, 150 us per launch at 65 536 rows).
+    // chunk's barrier wait and conversion: 8 warps x 16-32 requests of 128 bytes keep 16-32 KB in flight per SM.
     uint32_t it = 0;
     float cur[16], nxt[16];
     int item = blockIdx.x, c = 0;
@@ -195,120 +193,51 @@ __global__ void __launch_bounds__(kDtThreads, 1) dense_tc_rows_kernel(const __gr
       item = n_item;
       c = n_c;
     }
-  } else if (warp < 12) {
-    // ============================ epilogue: TMEM -> bias / act -> out ======================================
-    const int q = warp & 3;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    float* tb = tbuf + q * 32 * 17;
-    uint32_t cnt = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++cnt) {
-      const int mt = item / p.n_tiles, nt = item - mt * p.n_tiles;
-      const uint32_t buf = cnt & 1, par = (cnt >> 1) & 1;
-      tc::mbar_wait(&acc_full[buf], par);
-      tc::fence_after_thread_sync();
-      const int row_base = mt * 128 + q * 32;
-      const int n0 = nt * p.NT;
-      if (p.direct) {
-        // lane = output row: 32 accumulator columns per read, written as 8 float4 of the lane's own 128-byte line
-        // (no shared-memory transpose; the sectors of a line are completed by consecutive stores of the same lane)
-        const int grow = row_base + lane;
-        for (int cb = 0; cb * 32 < p.NT; ++cb) {
-          const int col0 = n0 + cb * 32;
-          if (col0 >= p.Nout) break;                             // warp-uniform
-          const bool second = cb * 32 + 16 < p.NT && col0 + 16 < p.Nout;
-          uint32_t v[2][16];
-          tc::tmem_ld16(tmem_base + lane_base + buf * kDtMaxNT + cb * 32, v[0]);
-          if (second) tc::tmem_ld16(tmem_base + lane_base + buf * kDtMaxNT + cb * 32 + 16, v[1]);
-          tc::tmem_wait_ld();
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (h == 1 && !second) break;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const int col = col0 + h * 16 + g * 4;
-              if (col >= p.Nout) break;                          // Nout % 4 == 0 on this path
-              float4 o = make_float4(__uint_as_float(v[h][4 * g]), __uint_as_float(v[h][4 * g + 1]),
-                                     __uint_as_float(v[h][4 * g + 2]), __uint_as_float(v[h][4 * g + 3]));
-              if (p.bias) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-                o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
-              }
-              if (p.act == DTB_ACT_RELU) {
-                o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-              } else if (p.act == DTB_ACT_TANH) {
-                o.x = tanhf(o.x); o.y = tanhf(o.y); o.z = tanhf(o.z); o.w = tanhf(o.w);
-              }
-              if (grow < p.M) *reinterpret_cast<float4*>(p.out + (int64_t)grow * p.ldo + col) = o;
-            }
-          }
-        }
-      } else
-      for (int cb = 0; cb * 16 < p.NT; ++cb) {
-        const int col0 = n0 + cb * 16;
-        if (col0 >= p.Nout) break;                               // warp-uniform
-        uint32_t v[16];
-        tc::tmem_ld16(tmem_base + lane_base + buf * kDtMaxNT + cb * 16, v);
-        tc::tmem_wait_ld();
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          float val = __uint_as_float(v[j]);
-          if (p.bias && col0 + j < p.Nout) val += __ldg(p.bias + col0 + j);
-          if (p.act == DTB_ACT_RELU) val = fmaxf(val, 0.f);
-          else if (p.act == DTB_ACT_TANH) val = tanhf(val);
-          tb[lane * 17 + j] = val;
-        }
-        __syncwarp();
-        const int col = lane & 15, hrow = lane >> 4;
-#pragma unroll
-        for (int rr = 0; rr < 16; ++rr) {
-          const int r = rr * 2 + hrow;
-          const int grow = row_base + r;
-          if (grow < p.M && col0 + col < p.Nout) p.out[(int64_t)grow * p.ldo + col0 + col] = tb[r * 17 + col];
-        }
-        __syncwarp();
-      }
-      tc::fence_before_thread_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_empty[buf]);
-    }
-  } else if (warp == 12) {
-    // ============================ MMA issue ==================================================================
-    const bool leader = dt_elect_one();
+  } else if (warp < 16) {
+    // ============================ MMA + epilogue: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile ====
+    const int wg = (warp >> 2) - 2;
+    const int wq = warp & 3;
     const uint32_t a_u32 = tc::smem_u32(smem_a), b_u32 = tc::smem_u32(smem_b);
-    const uint32_t idesc = tc::make_idesc_bf16(128, (uint32_t)p.NT);
-    const uint32_t lbo_b = (uint32_t)(p.NT >> 3) * 128;
-    const uint32_t img_b = (uint32_t)p.NT * kDtKc * 2;
-    uint32_t it = 0, cnt = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++cnt) {
-      const uint32_t buf = cnt & 1, par = (cnt >> 1) & 1;
-      tc::mbar_wait(&acc_empty[buf], par ^ 1);
-      tc::fence_after_thread_sync();
-      const uint32_t d_tmem = tmem_base + buf * kDtMaxNT;
+    uint32_t it = 0;
+    float acc[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int mt = item / p.n_tiles, nt = item - mt * p.n_tiles;
       for (int c = 0; c < p.n_chunks; ++c, ++it) {
         const uint32_t s = it % kDtStages, ph = (it / kDtStages) & 1;
         tc::mbar_wait(&full_b[s], ph);
         tc::mbar_wait(&full_a[s], ph);
-        tc::fence_after_thread_sync();
-        if (leader) {
-          const uint32_t a_addr = a_u32 + s * kDtAStage, b_addr = b_u32 + s * (uint32_t)lay.b_stage;
-#pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            // pass 0: A_hi*B_hi ; 1: A_lo*B_hi ; 2: A_hi*B_lo
-            const uint32_t a_img = a_addr + (pass == 1 ? kDtAImg : 0);
-            const uint32_t b_img = b_addr + (pass == 2 ? img_b : 0);
-#pragma unroll
-            for (int ks = 0; ks < kDtKc / 16; ++ks) {
-              const uint64_t da = tc::make_smem_desc(a_img + ks * 4096, 2048, 128);
-              const uint64_t db = tc::make_smem_desc(b_img + ks * 2 * lbo_b, lbo_b, 128);
-              tc::mma_ss(d_tmem, da, db, idesc, (uint32_t)((c | pass | ks) != 0));
-            }
-          }
-          tc::mma_commit(&empty[s]);
-        }
+        dt_mma_chunk<NT>(acc, a_u32 + s * kDtAStage, b_u32 + s * (uint32_t)lay.b_stage, wg, c == 0);
         __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&empty[s]);
       }
-      if (leader) tc::mma_commit(&acc_full[buf]);
-      __syncwarp();
+      const int row_a = mt * 128 + wg * 64 + wq * 16 + (lane >> 2);
+      const int n0 = nt * NT + 2 * (lane & 3);
+#pragma unroll
+      for (int i = 0; i < NT / 2; i += 2) {
+        const int grow = row_a + (((i >> 1) & 1) << 3);
+        const int col = n0 + 8 * (i >> 2);
+        if (grow >= p.M || col >= p.Nout) continue;
+        float o0 = acc[i], o1 = acc[i + 1];
+        const bool two = col + 1 < p.Nout;
+        if (p.bias) {
+          o0 += __ldg(p.bias + col);
+          if (two) o1 += __ldg(p.bias + col + 1);
+        }
+        if (p.act == DTB_ACT_RELU) {
+          o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f);
+        } else if (p.act == DTB_ACT_TANH) {
+          o0 = tanhf(o0); o1 = tanhf(o1);
+        }
+        float* dst = p.out + (int64_t)grow * p.ldo + col;
+        if (two && p.vec2) {
+          *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
+        } else {
+          dst[0] = o0;
+          if (two) dst[1] = o1;
+        }
+      }
     }
   } else {
     // ============================ weight loader ==============================================================
@@ -328,16 +257,10 @@ __global__ void __launch_bounds__(kDtThreads, 1) dense_tc_rows_kernel(const __gr
     }
     __syncwarp();
   }
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  if (warp == 12) {
-    tc::fence_after_thread_sync();
-    tc::tmem_dealloc(tmem_base, 512);
-  }
 }
 
 // ------------------------------------------------------------------------------------------
-// weight gradient: dW[k, n] += sum_m X[m, k] dZ[m, n].   UMMA M = 128 in-dim indices k (grid.x), N = NT out-dim indices
+// weight gradient: dW[k, n] += sum_m X[m, k] dZ[m, n].   MMA M = 128 in-dim indices k (grid.x), N = NT out-dim indices
 // (grid.z), reduction over batch rows in chunks of 32 (grid.y splits the batch).  Both operands are fp32 row-major
 // matrices whose ROWS are the reduction index: a lane reads the same column of two consecutive rows (coalesced across
 // the warp) and packs the pair into one K-major word.
@@ -350,7 +273,7 @@ struct DenseTcWgradParams {
   int M, K, N, ldx, ldz, ldw, NT, chunks_per_split, n_chunks_total;
 };
 
-// rows [m0, m0+32) x 4 column groups of 32 of src -> K-major image with UMMA row = column index, reduction index = row;
+// rows [m0, m0+32) x 4 column groups of 32 of src -> K-major image with MMA row = column index, reduction index = row;
 // this warp handles row pairs [pair0, pair0 + 4).  All 32 requests (4 groups x 4 pairs x 2 rows) are issued before the
 // first conversion.  Adds the column sums of the values it touched to colsum[] (for the bias gradient).
 __device__ __forceinline__ void dt_convert_cols4(const float* __restrict__ src, int ld, int m0, int m_valid, int col0,
@@ -386,41 +309,35 @@ __device__ __forceinline__ void dt_convert_cols4(const float* __restrict__ src, 
   }
 }
 
+template <int NT>
 __global__ void __launch_bounds__(kDtWgThreads, 1) dense_tc_wgrad_kernel(const __grid_constant__ DenseTcWgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const DtSmem lay = dt_layout(p.NT, 0);
+  const DtSmem lay = dt_layout(NT);
   uint8_t* smem_a = smem + lay.a_off;
   uint8_t* smem_b = smem + lay.b_off;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
   uint64_t* full = bars;                   // [stage] 8 producer warps
-  uint64_t* empty = bars + 4;              // [stage] commit
-  uint64_t* acc_done = bars + 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
+  uint64_t* empty = bars + 4;              // [stage] 8 consumer warps
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int k0 = blockIdx.x * 128, n0 = blockIdx.z * p.NT;
+  const int k0 = blockIdx.x * 128, n0 = blockIdx.z * NT;
   const int c_begin = blockIdx.y * p.chunks_per_split;
   int c_end = c_begin + p.chunks_per_split;
   if (c_end > p.n_chunks_total) c_end = p.n_chunks_total;
   const int n_ch = c_end > c_begin ? c_end - c_begin : 0;
-  const int b_img_bytes = p.NT * kDtKc * 2;
+  const int b_img_bytes = NT * kDtKc * 2;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kDtStages; ++s) {
       tc::mbar_init(&full[s], 8);
-      tc::mbar_init(&empty[s], 1);
+      tc::mbar_init(&empty[s], 8);
     }
-    tc::mbar_init(acc_done, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 8) tc::tmem_alloc(tmem_slot, 256);
-  tc::fence_before_thread_sync();
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 8) {
-    // warps 0-3: X -> A images (UMMA rows = k);  warps 4-7: dZ -> B images (UMMA rows = n); each warp owns 4 row pairs
+    // warps 0-3: X -> A images (MMA rows = k);  warps 4-7: dZ -> B images (MMA rows = n); each warp owns 4 row pairs
     const bool is_a = warp < 4;
     const int pair0 = (warp & 3) * 4;
     float bsum[kDtMaxNT / 32];
@@ -437,16 +354,7 @@ __global__ void __launch_bounds__(kDtWgThreads, 1) dense_tc_wgrad_kernel(const _
         dt_convert_cols4(p.X, p.ldx, m0, m_valid, k0, p.K, st, st + kDtAImg, 0, 128, pair0, lane, unused);
       } else {
         uint8_t* st = smem_b + s * lay.b_stage;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          if (half * 128 < p.NT) {
-            float cs[4] = {0.f, 0.f, 0.f, 0.f};
-            dt_convert_cols4(p.dZ, p.ldz, m0, m_valid, n0 + half * 128, p.N, st, st + b_img_bytes, half * 128, p.NT, pair0, lane,
-                             cs);
-#pragma unroll
-            for (int g = 0; g < 4; ++g) bsum[half * 4 + g] += cs[g];
-          }
-        }
+        dt_convert_cols4(p.dZ, p.ldz, m0, m_valid, n0, p.N, st, st + b_img_bytes, 0, NT, pair0, lane, bsum);
       }
       tc::fence_proxy_async_smem();
       __syncwarp();
@@ -456,77 +364,50 @@ __global__ void __launch_bounds__(kDtWgThreads, 1) dense_tc_wgrad_kernel(const _
 #pragma unroll
       for (int g = 0; g < kDtMaxNT / 32; ++g) {
         const int n = n0 + g * 32 + lane;
-        if (g * 32 < p.NT && n < p.N && bsum[g] != 0.f) atomicAdd(p.dbias + n, bsum[g]);
+        if (g * 32 < NT && n < p.N && bsum[g] != 0.f) atomicAdd(p.dbias + n, bsum[g]);
       }
     }
-    // ---- epilogue (warps 0-3, TMEM lane quadrant = warp): accumulator row = k -> dW[k, n0 ...] -----------------
-    if (is_a && n_ch > 0) {
-      tc::mbar_wait(acc_done, 0);
-      tc::fence_after_thread_sync();
-      const int k = k0 + warp * 32 + lane;
-      const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-      for (int cb = 0; cb * 16 < p.NT; ++cb) {
-        if (n0 + cb * 16 >= p.N) break;
-        uint32_t v[16];
-        tc::tmem_ld16(tmem_base + lane_base + cb * 16, v);
-        tc::tmem_wait_ld();
-        if (k < p.K) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int n = n0 + cb * 16 + j;
-            if (n < p.N) atomicAdd(p.dW + (int64_t)k * p.ldw + n, __uint_as_float(v[j]));
-          }
-        }
-      }
-      tc::fence_before_thread_sync();
-    }
-  } else if (warp == 8) {
-    const bool leader = dt_elect_one();
+  } else if (n_ch > 0) {
+    // ---- MMA + epilogue: warpgroup wg owns in-dim rows [k0 + 64 wg, k0 + 64 wg + 64) -> dW[k, n0 ...] -------------
+    const int wg = (warp >> 2) - 2;
     const uint32_t a_u32 = tc::smem_u32(smem_a), b_u32 = tc::smem_u32(smem_b);
-    const uint32_t idesc = tc::make_idesc_bf16(128, (uint32_t)p.NT);
-    const uint32_t lbo_b = (uint32_t)(p.NT >> 3) * 128;
+    float acc[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
     for (int c = 0; c < n_ch; ++c) {
       const uint32_t s = c % kDtStages, ph = (c / kDtStages) & 1;
       tc::mbar_wait(&full[s], ph);
-      tc::fence_after_thread_sync();
-      if (leader) {
-        const uint32_t a_addr = a_u32 + s * kDtAStage, b_addr = b_u32 + s * (uint32_t)lay.b_stage;
-#pragma unroll
-        for (int pass = 0; pass < 3; ++pass) {
-          const uint32_t a_img = a_addr + (pass == 1 ? kDtAImg : 0);
-          const uint32_t b_img = b_addr + (pass == 2 ? (uint32_t)b_img_bytes : 0);
-#pragma unroll
-          for (int ks = 0; ks < kDtKc / 16; ++ks) {
-            const uint64_t da = tc::make_smem_desc(a_img + ks * 4096, 2048, 128);
-            const uint64_t db = tc::make_smem_desc(b_img + ks * 2 * lbo_b, lbo_b, 128);
-            tc::mma_ss(tmem_base, da, db, idesc, (uint32_t)((c | pass | ks) != 0));
-          }
-        }
-        tc::mma_commit(&empty[s]);
-        if (c == n_ch - 1) tc::mma_commit(acc_done);
-      }
+      dt_mma_chunk<NT>(acc, a_u32 + s * kDtAStage, b_u32 + s * (uint32_t)lay.b_stage, wg, c == 0);
       __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&empty[s]);
     }
-  }
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  if (warp == 8) {
-    tc::fence_after_thread_sync();
-    tc::tmem_dealloc(tmem_base, 256);
+    const int k_a = k0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int n_a = n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) {
+      const int k = k_a + (((i >> 1) & 1) << 3);
+      const int n = n_a + 8 * (i >> 2) + (i & 1);
+      if (k < p.K && n < p.N) atomicAdd(p.dW + (int64_t)k * p.ldw + n, acc[i]);
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
+// wgmma N of a [*, Nout] output: the smallest supported width that holds it, else kDtMaxNT-wide column tiles
+static int dt_nt(int Nout) {
+  const int np = dt_round_up(Nout, 16);
+  return np <= 16 ? 16 : np <= 32 ? 32 : np <= 64 ? 64 : kDtMaxNT;
+}
+
 struct DtTiling {
   int NT, n_tiles, n_chunks;
 };
 static DtTiling dt_tiling(int K, int Nout) {
   DtTiling t;
-  const int np = dt_round_up(Nout, 16);
-  t.n_tiles = (np + kDtMaxNT - 1) / kDtMaxNT;
-  t.NT = dt_round_up((np + t.n_tiles - 1) / t.n_tiles, 16);
+  t.NT = dt_nt(Nout);
+  t.n_tiles = (Nout + t.NT - 1) / t.NT;
   t.n_chunks = (K + kDtKc - 1) / kDtKc;
   return t;
 }
@@ -534,6 +415,17 @@ static DtTiling dt_tiling(int K, int Nout) {
 size_t dense_tc_pack_bytes(int K, int Nout) {
   const DtTiling t = dt_tiling(K, Nout);
   return (size_t)t.n_tiles * t.n_chunks * t.NT * kDtKc * 4 + 256;
+}
+
+template <int NT>
+static int dt_launch_rows(const DenseTcRowsParams& p, int n_items, cudaStream_t st) {
+  const DtSmem lay = dt_layout(NT);
+  DTB_CUDA_OK(cudaFuncSetAttribute(dense_tc_rows_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+  int grid = sm_count();
+  if (grid > n_items) grid = n_items;
+  dense_tc_rows_kernel<NT><<<grid, kDtThreads, lay.total, st>>>(p);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
 }
 
 int dense_tc_rows(const float* A, int lda, const float* W, int ldw, int transposed, const float* bias, float* out,
@@ -555,18 +447,21 @@ int dense_tc_rows(const float* A, int lda, const float* W, int ldw, int transpos
   p.A = A; p.wpack = reinterpret_cast<const uint8_t*>(workspace); p.bias = bias; p.out = out;
   p.M = M; p.K = K; p.Nout = Nout; p.lda = lda; p.ldo = ldo; p.NT = t.NT; p.n_tiles = t.n_tiles; p.n_chunks = t.n_chunks;
   p.act = act;
-  {
-    static const int mode = [] { const char* e = getenv("DTB_DENSE_DIRECT"); return e ? atoi(e) : 1; }();   // 0: transposed
-    const bool ok = Nout % 4 == 0 && ldo % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
-                    (!bias || (reinterpret_cast<uintptr_t>(bias) & 15) == 0);
-    p.direct = (mode != 0 && ok) ? 1 : 0;
-  }
-  const DtSmem lay = dt_layout(t.NT, 1);
-  DTB_CUDA_OK(cudaFuncSetAttribute(dense_tc_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+  p.vec2 = (ldo % 2 == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0) ? 1 : 0;    // column pairs as one 8-byte store
   const int n_items = ((M + 127) / 128) * t.n_tiles;
-  int grid = sm_count();
-  if (grid > n_items) grid = n_items;
-  dense_tc_rows_kernel<<<grid, kDtThreads, lay.total, st>>>(p);
+  switch (t.NT) {
+    case 16: return dt_launch_rows<16>(p, n_items, st);
+    case 32: return dt_launch_rows<32>(p, n_items, st);
+    case 64: return dt_launch_rows<64>(p, n_items, st);
+    default: return dt_launch_rows<kDtMaxNT>(p, n_items, st);
+  }
+}
+
+template <int NT>
+static int dt_launch_wgrad(const DenseTcWgradParams& p, dim3 grid, cudaStream_t st) {
+  const DtSmem lay = dt_layout(NT);
+  DTB_CUDA_OK(cudaFuncSetAttribute(dense_tc_wgrad_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+  dense_tc_wgrad_kernel<NT><<<grid, kDtWgThreads, lay.total, st>>>(p);
   DTB_LAUNCH_OK();
   return DTB_OK;
 }
@@ -575,9 +470,8 @@ int dense_tc_wgrad(const float* X, int ldx, const float* dZ, int ldz, float* dW,
                    int N, cudaStream_t st) {
   if (M <= 0) return DTB_OK;
   DenseTcWgradParams p{};
-  const int np = dt_round_up(N, 16);
-  const int n_tiles = (np + kDtMaxNT - 1) / kDtMaxNT;
-  p.NT = dt_round_up((np + n_tiles - 1) / n_tiles, 16);
+  p.NT = dt_nt(N);
+  const int n_tiles = (N + p.NT - 1) / p.NT;
   p.X = X; p.dZ = dZ; p.dW = dW; p.dbias = dbias;
   p.M = M; p.K = K; p.N = N; p.ldx = ldx; p.ldz = ldz; p.ldw = ldw;
   p.n_chunks_total = (M + kDtKc - 1) / kDtKc;
@@ -587,11 +481,94 @@ int dense_tc_wgrad(const float* X, int ldx, const float* dZ, int ldz, float* dW,
   if (splits > p.n_chunks_total) splits = p.n_chunks_total;
   p.chunks_per_split = (p.n_chunks_total + splits - 1) / splits;
   splits = (p.n_chunks_total + p.chunks_per_split - 1) / p.chunks_per_split;
-  const DtSmem lay = dt_layout(p.NT, 0);
-  DTB_CUDA_OK(cudaFuncSetAttribute(dense_tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
-  dense_tc_wgrad_kernel<<<dim3(k_tiles, splits, n_tiles), kDtWgThreads, lay.total, st>>>(p);
+  const dim3 grid(k_tiles, splits, n_tiles);
+  switch (p.NT) {
+    case 16: return dt_launch_wgrad<16>(p, grid, st);
+    case 32: return dt_launch_wgrad<32>(p, grid, st);
+    case 64: return dt_launch_wgrad<64>(p, grid, st);
+    default: return dt_launch_wgrad<kDtMaxNT>(p, grid, st);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// tensor-core self test: C[128, N] = bf16(A[128, K]) . bf16(B[K, N]), one warpgroup, two m64 row blocks.  Isolates
+// descriptor / operand-layout mistakes from the GEMM pipelines above: B in the K-major image of the weight pack, A
+// either in the same image form (shared memory) or as register fragments.
+// ------------------------------------------------------------------------------------------
+template <int N, bool kARegs>
+__global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __restrict__ A, const float* __restrict__ Bm,
+                                                             float* __restrict__ C, int K) {
+  __shared__ __align__(128) uint8_t smem_b[N * 64 * 2];
+  __shared__ __align__(128) uint8_t smem_a[128 * 64 * 2];
+  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+  for (int e = t; e < K * N; e += 128) {
+    const int k = e / N, n = e - k * N;
+    const int off = ((k >> 3) * (N >> 3) + (n >> 3)) * 128 + (n & 7) * 16 + (k & 7) * 2;
+    *reinterpret_cast<__nv_bfloat16*>(smem_b + off) = __float2bfloat16_rn(Bm[e]);
+  }
+  if (!kARegs) {
+    for (int e = t; e < 128 * K; e += 128) {
+      const int r = e / K, k = e - r * K;
+      const int off = ((k >> 3) * 16 + (r >> 3)) * 128 + (r & 7) * 16 + (k & 7) * 2;
+      *reinterpret_cast<__nv_bfloat16*>(smem_a + off) = __float2bfloat16_rn(A[e]);
+    }
+  }
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+  float acc[2][N / 2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[h][i] = 0.f;
+  const int r0 = warp * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+  constexpr uint32_t lbo_b = (N >> 3) * 128;
+  tc::wgmma_fence();
+  for (int ks = 0; ks < K / 16; ++ks) {
+    const uint64_t db = tc::make_smem_desc(tc::smem_u32(smem_b) + ks * 2 * lbo_b, lbo_b, 128);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if constexpr (kARegs) {
+        const float* a = A + (int64_t)(h * 64 + r0) * K + ks * 16 + c0;
+        const uint32_t frag[4] = {tc::pack_bf16x2(a[0], a[1]), tc::pack_bf16x2(a[8 * K], a[8 * K + 1]),
+                                  tc::pack_bf16x2(a[8], a[9]), tc::pack_bf16x2(a[8 * K + 8], a[8 * K + 9])};
+        tc::Wgmma<N>::rs(acc[h], frag, db, ks != 0);
+      } else {
+        const uint64_t da = tc::make_smem_desc(tc::smem_u32(smem_a) + ks * 4096 + h * 1024, 2048, 128);
+        tc::Wgmma<N>::ss(acc[h], da, db, ks != 0);
+      }
+    }
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    tc::wgmma_fence_acc(acc[h]);
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i)
+      C[(h * 64 + r0 + (((i >> 1) & 1) << 3)) * N + 8 * (i >> 2) + c0 + (i & 1)] = acc[h][i];
+  }
+}
+
+template <int N>
+static int tc_selftest_launch(const float* A, const float* Bm, float* C, int K, int a_regs, cudaStream_t st) {
+  if (a_regs) tc_selftest_kernel<N, true><<<1, 128, 0, st>>>(A, Bm, C, K);
+  else tc_selftest_kernel<N, false><<<1, 128, 0, st>>>(A, Bm, C, K);
   DTB_LAUNCH_OK();
   return DTB_OK;
 }
 
 }  // namespace dtb
+
+extern "C" int dtb_tc_selftest(const float* A, const float* Bmat, float* C, void* workspace, int N, int K,
+                               int a_operand_in_regs, void* stream) {
+  DTB_CHECK_ARG(A && Bmat && C && workspace, "NULL argument");
+  DTB_CHECK_ARG((N == 16 || N == 32 || N == 64 || N == 128) && K % 16 == 0 && K >= 16 && K <= 64,
+                "N in {16, 32, 64, 128}, K <= 64 a multiple of 16");
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (N) {
+    case 16: return dtb::tc_selftest_launch<16>(A, Bmat, C, K, a_operand_in_regs, st);
+    case 32: return dtb::tc_selftest_launch<32>(A, Bmat, C, K, a_operand_in_regs, st);
+    case 64: return dtb::tc_selftest_launch<64>(A, Bmat, C, K, a_operand_in_regs, st);
+    default: return dtb::tc_selftest_launch<128>(A, Bmat, C, K, a_operand_in_regs, st);
+  }
+}

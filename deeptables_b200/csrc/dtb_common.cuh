@@ -1,4 +1,4 @@
-// Shared helpers for the deeptables_b200 sm_100a kernels.
+// Shared helpers for the deeptables_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

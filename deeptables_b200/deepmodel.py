@@ -1,11 +1,11 @@
-"""DeepModel -- the reference's model object (deeptables/models/deepmodel.py) on the B200 engine.
+"""DeepModel -- the reference's model object (deeptables/models/deepmodel.py) on the H100 engine.
 
 Same constructor and public methods (fit / predict / evaluate / apply / save / release, attributes
 ``model``, ``model_desc``, ``config``), same graph (``__build_model``, reference deepmodel.py:259-317:
 inputs -> MultiColumnEmbedding -> flatten/concat + BatchNormalization -> net builders -> stacking ->
 ``task_output``), same training contract (Adam(1e-3) + BCE/MSE/CCE when ``optimizer``/``loss`` are
 'auto', reference deepmodel.py:319-346; ``steps_per_epoch`` / ``validation_steps`` arithmetic,
-reference deepmodel.py:76-83).  The numerics run in hand-written sm_100a kernels behind the C ABI;
+reference deepmodel.py:76-83).  The numerics run in hand-written sm_90a kernels behind the C ABI;
 torch supplies device memory and the autograd tape only.
 
 Multi-GPU: one process per GPU under ``torch.distributed`` (NCCL).  Each rank trains on its shard
@@ -235,7 +235,7 @@ class DeepModel:
         self._seed = seed
         self._step = 0
         if not torch.cuda.is_available():
-            raise RuntimeError('deeptables_b200 needs a CUDA device (sm_100a); there is no CPU path')
+            raise RuntimeError('deeptables_b200 needs a CUDA device (H100, sm_90a); there is no CPU path')
         if device is None:
             device = torch.device('cuda', torch.cuda.current_device())
         self.device = torch.device(device)

@@ -163,7 +163,7 @@ def autoint_nets(embeddings, flatten_emb_layer, dense_layer, concat_emb_dense, c
 
 def _out_of_scope(name):
     def fn(embeddings, flatten_emb_layer, dense_layer, concat_emb_dense, config, model_desc):
-        raise NotImplementedError(f'{name} is outside the B200 hot path of this build (SURVEY.md 8f)')
+        raise NotImplementedError(f'{name} is outside the hot path of this build (SURVEY.md 8f)')
     fn.__name__ = name
     return fn
 

@@ -1,5 +1,5 @@
 """DeepTable -- the user-facing estimator of the reference (deeptables/models/deeptable.py) over the
-B200 engine: ``DeepTable(config).fit(X, y) / predict / predict_proba / evaluate / save / load``.
+H100 engine: ``DeepTable(config).fit(X, y) / predict / predict_proba / evaluate / save / load``.
 
 The train/score hot path (DeepModel) is the product; what surrounds it here is the thinnest host
 layer that makes the README flow work on a pandas DataFrame: a pandas/sklearn ``DefaultPreprocessor``

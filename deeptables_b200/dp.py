@@ -1,7 +1,7 @@
 """Data-parallel gradient exchange (reference: tf.distribute.MirroredStrategy around the model
 build, deepmodel.py:88-103 -- gradient all-reduce inside TensorFlow, per-replica BatchNorm).
 
-One process per GPU, ``torch.distributed`` (NCCL over NVLink on the B200 box; gloo in the CPU tests).
+One process per GPU, ``torch.distributed`` (NCCL between the GPUs of one machine; gloo in the CPU tests).
 The path shards by batch rows only, so the exchange is:
 
   1. the loss gradient is pre-scaled by 1/world_size (``scale_for_mean``), which turns the SUM

@@ -1,5 +1,5 @@
 """Interaction layers with the reference's names and constructor arguments
-(reference deeptables/models/layers.py), executed by hand-written sm_100a kernels through the
+(reference deeptables/models/layers.py), executed by hand-written sm_90a kernels through the
 C ABI.  Layers are define-by-run: calling one inside a model scope creates (first call) or looks
 up (later calls) its weights under the Keras-style layer name, so net builders -- the built-in
 ones in deepnets.py and user callables with the same 6-argument signature -- read exactly like
@@ -400,7 +400,7 @@ class InnerOuterProduct(Layer):
 def _out_of_scope(name):
     class _Stub(Layer):
         def __init__(self, *a, **k):
-            raise NotImplementedError(f'{name} is outside the B200 hot path of this build '
+            raise NotImplementedError(f'{name} is outside the hot path of this build '
                                       f'(SURVEY.md 8f): not implemented')
     _Stub.__name__ = name
     return _Stub

@@ -1,5 +1,5 @@
 /*
- * deeptables_b200 -- C ABI of the B200-native feature-interaction engine.
+ * deeptables_b200 -- C ABI of the H100-native (sm_90a) feature-interaction engine.
  *
  * The reference (DataCanvasIO/DeepTables) has no native boundary at all: every op below is, in
  * the reference, a chain of TensorFlow/Keras ops inside a Keras layer (file:line cited per
@@ -101,9 +101,9 @@ int dtb_batchnorm_bwd(const float* X, const float* dY, float* dX, const float* g
 
 /* ---- Dense (keras Dense used by deepnets.dnn 415-424, stacking 292, task_output 455; the four
  * projections of MultiheadAttention, layers.py:106-127) ----------------------------------------- */
-/* Layers wider than 8 outputs run as hand-written tcgen05 GEMMs (csrc/dense_tc.cu: operands split on the fly into
- * bf16 hi + lo, three tensor passes, fp32 accumulation in TMEM => fp32-grade results; bias / activation fused into the
- * accumulator read-out); out_dim <= 8 (logit layers) as row-dot kernels.  The GEMM path packs the weights into
+/* Layers wider than 8 outputs run as hand-written wgmma GEMMs (csrc/dense_tc.cu: operands split on the fly into
+ * bf16 hi + lo, three tensor passes, fp32 accumulation in registers => fp32-grade results; bias / activation fused into
+ * the accumulator read-out); out_dim <= 8 (logit layers) as row-dot kernels.  The GEMM path packs the weights into
  * `workspace` (dtb_dense_workspace_bytes(in_dim, out_dim), 16-byte aligned; 0 for the narrow kernels). */
 size_t dtb_dense_workspace_bytes(int in_dim, int out_dim);
 /* Y[rows,out] = act(X[rows,in] @ W[in,out] + bias).  bias may be NULL. */
@@ -216,27 +216,28 @@ int dtb_cin_bwd_phase(const int32_t* idx, const float* table, const int64_t* row
                       float* d_weights, float* d_bias, void* workspace, size_t workspace_bytes, int B, int F,
                       int D, const int* layer_sizes_host, int n_layers, int direct, int act, int precision,
                       int phase, void* stream);
-/* precision:
- *   0 = auto: ONE tensor pass on fp16 operands scaled by exact powers of two (per GEMM row / per layer; csrc/cin_tc2.cu:
- *       forward, data gradient and weight gradient, embedding dim 16 or 32, layer sizes multiples of 32, <= 64 hidden
- *       fields) -- error ~2e-4 of the output scale, inside the 1e-3 parity bar; shapes outside it fall to 2, then to 1;
+/* precision (forward; codes 2-4 share the fused bf16x3 backward of csrc/cin_wgmma.cu, code 1 the any-shape backward):
+ *   0 = auto: 2 where dtb_cin_tc_supported(), else 1;
  *   1 = the any-shape materialising formulation (outer product in HBM chunks + the bf16x3 GEMMs of csrc/dense_tc.cu);
- *   2 = tensor-core bf16x3 split (hi*hi + lo*hi + hi*lo, ~2^-16 per product: fp32-grade); 3 = one bf16 pass (4e-3: tests only);
- *   4 = force the single fp16 pass (error when the shape is outside it). */
+ *   2 = fused wgmma forward (csrc/cin_wgmma.cu: embedding dim 4/8/16/32, <= 64 fields, <= 64 hidden fields and <= 128
+ *       feature maps per layer), bf16x3 split: fp32-grade; 3 = the same with one bf16 pass; 4 = one pass on fp16
+ *       operands scaled by exact powers of two.  Codes 2-4 return DTB_ERR_UNSUPPORTED outside the fused shapes. */
 #define DTB_CIN_AUTO 0
 #define DTB_CIN_FP32 1
 #define DTB_CIN_TC_BF16X3 2
 #define DTB_CIN_TC_BF16X1 3
 #define DTB_CIN_TC_F16X1 4
 int dtb_cin_tc_supported(int F, int D, const int* layer_sizes_host, int n_layers, int direct);
-/* which of the codes 1 / 2 / 4 a forward + backward with `precision` runs for this shape (0 = auto is resolved) */
+/* which of the codes 1-4 a forward + backward with `precision` runs for this shape (0 = auto is resolved) */
 int dtb_cin_resolved_precision(int F, int D, const int* layer_sizes_host, int n_layers, int direct, int precision);
-/* Test hooks for the tensor-core path.  set_variant: 1 (default) feeds the on-the-fly A operand to
- * tcgen05.mma through TMEM, 0 through shared memory.  selftest: C[128,N] = bf16(A[128,K]) @
- * bf16(Bmat[K,N]) with one M=128 UMMA tile (N <= 128, K <= 64, multiples of 16); workspace >= 4*N*K bytes. */
-int dtb_cin_tc_set_variant(int a_operand_in_tmem);
+/* Test hooks for the tensor-core path.  set_variant: bit 16 set runs the any-shape backward (exact-fp32 outer product)
+ * instead of the fused one after a fused forward; every other bit is ignored (they chose between kernel variants of
+ * the earlier sm_100a build).  selftest: C[128,N] = bf16(A[128,K]) @ bf16(Bmat[K,N]) on one warpgroup
+ * (two m64 wgmma row blocks; N in {16, 32, 64, 128}, K <= 64 a multiple of 16), the A operand from registers
+ * (a_operand_in_regs = 1) or from shared memory (0); workspace is not used and may be any non-NULL pointer. */
+int dtb_cin_tc_set_variant(int variant);
 int dtb_tc_selftest(const float* A, const float* Bmat, float* C, void* workspace, int N, int K,
-                    int a_operand_in_tmem, void* stream);
+                    int a_operand_in_regs, void* stream);
 
 /* ---- Cross (layers.py:417-436) on a dense [B,W] input ------------------------------------- */
 /* x_{l+1} = x0*(x_l . w_l) + x_l + b_l ; kernels/biases [n_layers, W]; Y [B,W].

@@ -1,7 +1,7 @@
 """Data-parallel training on 2 (and, when the box has them, 8) GPUs over NCCL: replicas stay bit-identical -- weights
 after 6 optimiser steps and, once averaged (DeepModel.sync_replica_buffers, MirroredStrategy's MEAN aggregation), the
 BatchNormalization moving statistics -- and ranks fed the SAME shard reproduce the single-GPU run on that shard (mean
-of identical gradients).  profiles/r2_dp_nccl_tests.log holds the round-2 run of this file on 2 and 8 B200s."""
+of identical gradients).  With fewer than 2 GPUs the tests skip."""
 import os
 import socket
 

@@ -197,7 +197,7 @@ def test_concat_and_batchnorm(nat, vocab, d, c, b):
     np.testing.assert_allclose(gt.cpu().numpy(), want_g, rtol=1e-5, atol=1e-6)
 
 
-# wide layers = tcgen05 GEMMs (dense_tc.cu): tower shapes, 1079-wide PNN input, AutoInt projection (32 -> 128), ragged
+# wide layers = wgmma GEMMs (dense_tc.cu): tower shapes, 1079-wide PNN input, AutoInt projection (32 -> 128), ragged
 # row counts / odd widths, more than one 256-column output tile (dX of the 1079-wide layer), K smaller than one chunk
 @pytest.mark.parametrize('rows,i,o,act', [(300, 429, 128, 1), (300, 128, 64, 1), (77, 64, 1, 0), (50, 1, 1, 0),
                                            (64, 37, 3, 0), (5, 10, 20, 1), (1000, 1079, 128, 1), (2600, 32, 128, 1),
@@ -217,7 +217,7 @@ def test_dense_fwd_bwd(nat, rows, i, o, act):
     w64 = torch.tensor(w, dtype=torch.float64, requires_grad=True)
     b64 = torch.tensor(bias, dtype=torch.float64, requires_grad=True)
     y64 = L.dense(x64, w64, b64, 'relu' if act else None)
-    # out_dim > 8: tcgen05 GEMM on bf16 hi/lo splits (three passes, the dropped lo*lo term is 2^-16 of a product): a
+    # out_dim > 8: wgmma GEMM on bf16 hi/lo splits (three passes, the dropped lo*lo term is 2^-16 of a product): a
     # few 1e-5 absolute on O(1) outputs; the narrow kernels are plain fp32
     tc = o > 8
     np.testing.assert_allclose(Y.cpu().numpy(), y64.detach().numpy(), rtol=1e-4, atol=1e-4 if tc else 1e-5)
@@ -226,7 +226,7 @@ def test_dense_fwd_bwd(nat, rows, i, o, act):
     dW = torch.zeros(i, o, device='cuda')
     dB = torch.zeros(o, device='cuda')
     # the backward takes the relu mask from Y: hand it the oracle's Y, otherwise an output whose pre-activation lies within
-    # the forward's rounding error of zero flips its mask bit and a whole row of dX moves by |dy . W| (seen on the B200
+    # the forward's rounding error of zero flips its mask bit and a whole row of dX moves by |dy . W| (seen on the GPU
     # at 128 000+ outputs: one such element) -- that is the forward's tolerance, not the backward's arithmetic
     Yb = dev(y64.detach().numpy().astype(np.float32))
     nat.check(nat.lib.dtb_dense_bwd(P(X), P(W), P(Yb), P(dY), P(dX), P(dW), P(dB), P(ws), wsb, rows, i, o, act, None))
@@ -498,7 +498,7 @@ def test_cross_fwd_bwd(nat, b, w, n):
 
 
 # ---------------------------------------------------------------------------------------------
-# tensor-core (tcgen05) path
+# tensor-core (wgmma) path
 # ---------------------------------------------------------------------------------------------
 def _bf16(x):
     return torch.tensor(x).to(torch.bfloat16).to(torch.float32).numpy()
@@ -507,8 +507,9 @@ def _bf16(x):
 @pytest.mark.parametrize('a_in_tmem', [1, 0])
 @pytest.mark.parametrize('n,k', [(128, 64), (32, 16), (64, 32)])
 def test_tc_selftest_gemm(nat, a_in_tmem, n, k):
-    """One M=128 UMMA tile: validates the instruction / shared-memory descriptors, the TMEM
-    operand layout and the accumulator read-back against an exact bf16-input reference."""
+    """One 128-row wgmma tile: validates the shared-memory descriptors, the register-fragment layout of the A operand
+    (a_in_tmem = 1: A from registers, Hopper's counterpart of an A operand in tensor memory) and the accumulator
+    read-back against an exact bf16-input reference."""
     g = np.random.default_rng(20)
     a = g.normal(size=(128, k)).astype(np.float32)
     bm = g.normal(size=(k, n)).astype(np.float32)
@@ -531,7 +532,7 @@ TC_CASES = [  # (F, D, sizes, direct, bias, act, B)
 
 
 @pytest.mark.parametrize('f,d,sizes,direct,use_bias,act,b', TC_CASES)
-@pytest.mark.parametrize('variant', [1, 0])
+@pytest.mark.parametrize('variant', [1, 0])      # sm_100a kernel variants; the sm_90a build ignores it (one kernel)
 @pytest.mark.parametrize('precision', [2, 3])
 def test_cin_tensor_core_forward(nat, f, d, sizes, direct, use_bias, act, b, variant, precision):
     sizes_c = nat.int_array(sizes)
@@ -607,7 +608,7 @@ def test_cin_tensor_core_full_batch_properties(nat):
 
 @pytest.mark.parametrize('f,d,sizes,direct,use_bias,act,b', TC_CASES)
 def test_cin_tensor_core_backward(nat, f, d, sizes, direct, use_bias, act, b):
-    """dgrad + wgrad on tcgen05 (bf16x3) against the oracle's autograd."""
+    """dgrad + wgrad on the fused wgmma kernels (bf16x3) against the any-shape backward and the oracle's autograd."""
     sizes_c = nat.int_array(sizes)
     n = len(sizes)
     if not nat.lib.dtb_cin_tc_supported(f, d, sizes_c, n, int(direct)):
@@ -641,18 +642,14 @@ def test_cin_tensor_core_backward(nat, f, d, sizes, direct, use_bias, act, b):
         torch.cuda.synchronize()
         return gt_, dw_, db_
 
-    # (0) default = compact saved activations (relu-mask bits + the operand tiles); bit 17 keeps the fp32 T_k
-    #     rows.  Same arithmetic on the same values: only the order of the fp32 atomics may differ.
+    # (0) the sm_90a build has one saved-activation format (bit 17 of set_variant, which chose between two on sm_100a,
+    #     is ignored): two runs must agree up to the order of the fp32 atomics.
     gt_c, dw_c, db_c = fwd_bwd()
-    nat.lib.dtb_cin_tc_set_variant(1 | (1 << 17))
-    try:
-        gt, dw, dbias = fwd_bwd()
-    finally:
-        nat.lib.dtb_cin_tc_set_variant(1)
+    gt, dw, dbias = fwd_bwd()
     for a_, b_, what in ((gt_c, gt, 'embedding grad'), (dw_c, dw, 'filter grad'), (db_c, dbias, 'bias grad')):
         if a_ is not None:
             e = float((a_ - b_).abs().max() / b_.abs().max())
-            assert e < 2e-6, f'compact vs full saved activations, {what}: {e:.2e}'
+            assert e < 2e-6, f'two runs of the fused backward, {what}: {e:.2e}'
     # (1) same saved activations (=> identical relu masks) through the exact-fp32 backward: the two
     #     backward implementations must agree to bf16x3 precision
     gt2 = torch.zeros(flat.shape, device='cuda')
@@ -858,7 +855,7 @@ def test_fgcnn_conv_and_pool_fwd_bwd(nat, b, h, w, cin, cout, kh, pool, act):
 
 
 def test_dense_tanh_activation(nat):
-    """DTB_ACT_TANH in the Dense epilogues (wide: tcgen05 path, narrow: row-dot path) and its backward."""
+    """DTB_ACT_TANH in the Dense epilogues (wide: wgmma path, narrow: row-dot path) and its backward."""
     g = np.random.default_rng(82)
     for rows, i, o in ((300, 36, 40), (200, 48, 5)):
         x = g.normal(size=(rows, i)).astype(np.float32)
