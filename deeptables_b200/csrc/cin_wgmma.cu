@@ -11,7 +11,10 @@
 // Precision: 2 = bf16x3 split (Z_hi W_hi + Z_lo W_hi + Z_hi W_lo: fp32-grade), 3 = one bf16 pass, 4 = one fp16 pass on
 // operands scaled by exact powers of two (per GEMM row for Z, per layer for W_k), undone on the fp32 accumulator.
 // The saved activations have the layout of the any-shape formulation (x0t, then T_k).  The backward (below) runs the
-// data and weight gradients as two fused wgmma kernels in bf16x3 for every precision code.
+// data and weight gradients as two fused wgmma kernels in bf16x3 for every precision code.  The data-gradient kernel
+// (one warpgroup per CTA, like the forward) hands dC_k to the weight-gradient kernel already split into the bf16 hi/lo
+// image wgmma reads; the weight-gradient CTA is two warpgroups that share each bulk-copied 64-row block among four
+// m64 A tiles (one or two x0 fields each).
 #include "dtb_common.cuh"
 #include "cin_impl.h"
 #include "wgmma.cuh"
@@ -286,11 +289,19 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
 //     dC_k = (d_pooled part + dh_{k+1}) * act'(T_k)                 registers, accumulator fragment layout
 //     dZ_{k,i}[m, j] = sum_l dC_k[m, l] W_k[i*H + j, l]             wgmma: A = dC_k from registers, B = W_k^T chunk
 //     dx0[m, i] += sum_j dZ h_k[m, j] ;  dh_k[m, j] += dZ x0[m, i]   registers (dh_k feeds dC_{k-1})
-//     dC_k is stored (fp32) for the weight gradient; dx0 is scattered into grad_table.
-//   wgrad, per (layer k, x0 field i, row split):
+//     dC_k is stored as the bf16 hi/lo image the weight gradient multiplies (below), its column sums go to d_bias,
+//     and dx0 is scattered into grad_table.
+//   wgrad, per (layer k, group of x0 fields, row split):
 //     dW_k[i*H + j, l] += sum_m x0[m, i] h_k[m, j] dC_k[m, l]       wgmma: A = x0 h from registers (rows j),
 //                                                                   B = dC_k block as a K-major image (K = m)
+//     Two warpgroups x two m64 A tiles per CTA: one bulk copy of each 64-row block (dC_k image, x0 rows, h_k rows)
+//     into a two-stage ring serves four tiles.  A tile holds one field (H > 32) or two (rows 0-31 and 32-63).
 // ==========================================================================================
+
+// dC_k of one 64-row block: K-major image (K = m, N = l < NP) of bf16 hi then lo, core (m/8, l/8) at
+// ((m/8)*(NP/8) + l/8)*128 B, row l%8 at 16 B, element m%8 at 2 B.  Zero past L_k and past the last row.
+__host__ __device__ inline uint32_t cin_wg_dc_block_bytes(int NP) { return (uint32_t)NP * kWgRows * 4; }
+
 struct CinWgBwdParams {
   const int32_t* idx;
   const int64_t* row_offsets;
@@ -298,11 +309,12 @@ struct CinWgBwdParams {
   const float* d_pooled;
   const float* saved;        // x0t [B*D, F] then T_k [B*D, L_k]
   float* grad_table;
-  float* dc;                 // dC_k [B*D, L_k] per layer
-  int B, D, F, n_layers, act, P;
+  uint8_t* dc;               // dC_k images, per layer, per 64-row block (cin_wg_dc_block_bytes(NPdc))
+  float* dbias;              // null, or d_bias of all layers (offsets bias_off)
+  int B, D, F, n_layers, act, P, NPdc;
   int L[kCinMaxLayers], LP[kCinMaxLayers], H[kCinMaxLayers], hid_n[kCinMaxLayers];
   int pool_lo[kCinMaxLayers], pool_n[kCinMaxLayers], pcol0[kCinMaxLayers];
-  unsigned long long wpack_off[kCinMaxLayers], saved_off[kCinMaxLayers], dc_off[kCinMaxLayers];
+  unsigned long long wpack_off[kCinMaxLayers], saved_off[kCinMaxLayers], dc_off[kCinMaxLayers], bias_off[kCinMaxLayers];
 };
 
 // W_k [F*H, L] -> per field i: K-major image of B[n][kk] = W_k[i*H + n, kk] (n < H, kk < L, else 0), N = NPJ, K = LP
@@ -324,14 +336,15 @@ __global__ void cin_wg_pack_t_kernel(const float* __restrict__ w, uint8_t* __res
 }
 
 struct CinWgBwdSmem {
-  int w_off, x0_off, dx_off, bar_off, total;
+  int w_off, x0_off, dx_off, bsum_off, bar_off, total;
 };
 __host__ __device__ inline CinWgBwdSmem cin_wg_bwd_layout(int NPJ, int F) {
   CinWgBwdSmem l;
   l.w_off = 0;
   l.x0_off = 2 * NPJ * kWgMaxNP * 4;                 // two W^T chunk buffers (hi + lo)
   l.dx_off = l.x0_off + kWgRows * F * 4;
-  l.bar_off = (l.dx_off + kWgRows * F * 4 + 15) / 16 * 16;
+  l.bsum_off = l.dx_off + kWgRows * F * 4;           // this CTA's d_bias partial sums [layer][l]
+  l.bar_off = (l.bsum_off + kCinMaxLayers * kWgMaxNP * 4 + 15) / 16 * 16;
   l.total = l.bar_off + 16;
   return l;
 }
@@ -344,6 +357,7 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
   uint8_t* wbuf = smem + lay.w_off;
   float* x0s = reinterpret_cast<float*>(smem + lay.x0_off);      // [m][i]
   float* dxs = reinterpret_cast<float*>(smem + lay.dx_off);      // [m][i]
+  float* bsum = reinterpret_cast<float*>(smem + lay.bsum_off);   // [k][l]
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int F = p.F, D = p.D;
@@ -352,6 +366,11 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
   const int r0 = warp * 16 + (lane >> 2), c2 = 2 * (lane & 3);
   constexpr uint32_t lbo_b = (NPJ >> 3) * 128;
   const int K0 = p.n_layers - 1;
+  const int NPdc = p.NPdc;
+  const uint32_t dc_img = NPdc * kWgRows * 2;                     // bytes of the hi (and of the lo) image of a block
+  const bool do_bias = p.dbias != nullptr;
+  const bool odd_row = (lane >> 2) & 1;
+  for (int e = tid; e < kCinMaxLayers * kWgMaxNP; e += 128) bsum[e] = 0.f;
 
   if (tid == 0) {
     tc::mbar_init(&full[0], 1);
@@ -384,7 +403,8 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
       uint32_t ahi[kWgMaxNP / 16][4], alo[kWgMaxNP / 16][4];
       {
         const float* T = p.saved + p.saved_off[k];
-        float* dcg = p.dc + p.dc_off[k];
+        uint8_t* img = p.dc + p.dc_off[k] + (size_t)tile * cin_wg_dc_block_bytes(NPdc);
+        float bs[2] = {0.f, 0.f};
 #pragma unroll
         for (int q = 0; q < kWgMaxNP / 2; q += 2) {
           const int row = r0 + (((q >> 1) & 1) << 3), l = 8 * (q >> 2) + c2;
@@ -400,11 +420,41 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
                   g[u] += __ldg(p.d_pooled + b * p.P + p.pcol0[k] + lu - p.pool_lo[k]);
                 if (lu < p.hid_n[k] && q + u < NPJ / 2) g[u] += dh[q + u];
                 if (p.act == DTB_ACT_RELU && !(T[gm * L + lu] > 0.f)) g[u] = 0.f;
-                dcg[gm * L + lu] = g[u];
               }
             }
           }
           tc::split_bf16x2(g[0], g[1], ahi[q >> 3][(q >> 1) & 3], alo[q >> 3][(q >> 1) & 3]);
+          // dC image: the lane of the partner row (lane ^ 4) swaps one value, so each lane holds rows (2t, 2t + 1) of
+          // one column and stores their hi and lo pairs as one word each.  Only the stores are conditional: a branch
+          // around the register work would make ptxas serialize the wgmma that follow.
+          {
+            const float other = __shfl_xor_sync(0xffffffffu, odd_row ? g[0] : g[1], 4);
+            const float z0 = odd_row ? other : g[0], z1 = odd_row ? g[1] : other;
+            const int mr = odd_row ? row - 1 : row, lc = odd_row ? l + 1 : l;
+            uint32_t hi, lo;
+            tc::split_bf16x2(z0, z1, hi, lo);
+            const uint32_t off = ((mr >> 3) * (NPdc >> 3) + (lc >> 3)) * 128 + (lc & 7) * 16 + (mr & 7) * 2;
+            if (l < NPdc) {
+              *reinterpret_cast<uint32_t*>(img + off) = hi;
+              *reinterpret_cast<uint32_t*>(img + dc_img + off) = lo;
+            }
+          }
+          // d_bias: q and q + 2 are rows r0 and r0 + 8 of the same columns; then the sum over the 8 row lanes
+          if (do_bias) {
+            if ((q & 2) == 0) {
+              bs[0] = g[0];
+              bs[1] = g[1];
+            } else {
+#pragma unroll
+              for (int u = 0; u < 2; ++u) {
+                float v = bs[u] + g[u];
+                v += __shfl_xor_sync(0xffffffffu, v, 4);
+                v += __shfl_xor_sync(0xffffffffu, v, 8);
+                v += __shfl_xor_sync(0xffffffffu, v, 16);
+                if (lane < 4 && l + u < L && v != 0.f) atomicAdd(&bsum[k * kWgMaxNP + l + u], v);
+              }
+            }
+          }
         }
       }
       // h_k in fragment order (columns j), and the fresh dh_k accumulators
@@ -486,90 +536,153 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
     }
     __syncthreads();
   }
+  if (do_bias) {
+    for (int e = tid; e < p.n_layers * kWgMaxNP; e += 128) {
+      const int k = e / kWgMaxNP, l = e - k * kWgMaxNP;
+      if (l < p.L[k] && bsum[e] != 0.f) atomicAdd(p.dbias + p.bias_off[k] + l, bsum[e]);
+    }
+  }
 }
 
 struct CinWgWgradParams {
   const float* x0t;      // [B*D, F]
-  const float* h;        // h_k rows: x0t (k = 0) or T_{k-1}, leading dimension ldh
-  const float* dc;       // dC_k [B*D, L]
+  const float* h;        // T_{k-1} [B*D, ldh] (its first H columns are h_k); null for k = 0, where h_0 = x0
+  const uint8_t* dc;     // dC_k images, one per 64-row block
   float* dw;             // dW_k [F*H, L]
-  float* dbias;          // [L] or null
   int64_t BD;
   int F, H, L, ldh, blocks_per_split;
+  int fields_per_tile;   // 2: rows 0-31 of an A tile are field 2t, rows 32-63 field 2t + 1 (H <= 32); else 1
+  int hpitch;            // floats between h rows in shared memory
+  int hrow_bytes;        // > 0: h rows are copied one by one (that many bytes, to the padded pitch); 0: as one block
 };
 
+constexpr int kWgradTiles = 4;          // A tiles per CTA: two warpgroups x two m64 accumulators
+
+struct CinWgWgradSmem {
+  int x0_off, h_off, stage, bar_off, total;
+};
+__host__ __device__ inline CinWgWgradSmem cin_wg_wgrad_layout(int NP, int F, int hpitch) {
+  CinWgWgradSmem l;
+  l.x0_off = (int)cin_wg_dc_block_bytes(NP);
+  l.h_off = l.x0_off + (kWgRows * F * 4 + 127) / 128 * 128;
+  l.stage = l.h_off + (kWgRows * hpitch * 4 + 127) / 128 * 128;
+  l.bar_off = 2 * l.stage;
+  l.total = l.bar_off + 16;
+  return l;
+}
+
 template <int NP>
-__global__ void __launch_bounds__(128) cin_wg_wgrad_kernel(const __grid_constant__ CinWgWgradParams p) {
+__global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_constant__ CinWgWgradParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* bimg = smem;                                                          // dC block, K-major (K = m), hi | lo
-  float (*hs)[kWgMaxHp + 1] = reinterpret_cast<float (*)[kWgMaxHp + 1]>(smem + 2 * NP * kWgRows * 2);
-  float* xs = reinterpret_cast<float*>(smem + 2 * NP * kWgRows * 2 + kWgRows * (kWgMaxHp + 1) * 4);
-  float* bsum = xs + kWgRows;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int i = blockIdx.x;
-  const int j0 = warp * 16 + (lane >> 2), c2 = 2 * (lane & 3);           // A rows j0, j0 + 8; k columns m
+  const CinWgWgradSmem lay = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
+  const int c2 = 2 * (lane & 3);
   constexpr uint32_t lbo_b = (NP >> 3) * 128;
   constexpr uint32_t img = NP * kWgRows * 2;
-  const bool do_bias = p.dbias && i == 0;
-  for (int l = tid; l < NP; l += 128) bsum[l] = 0.f;
-  float acc[NP / 2];
+  const int F = p.F, H = p.H;
+  // this warp's 16 A rows belong to one field of each of its warpgroup's two tiles; the thread's rows are jw, jw + 8
+  const int upper = p.fields_per_tile == 2 && wq >= 2;
+  const int jw = (wq - 2 * upper) * 16 + (lane >> 2);
+  int field[2];
+  bool tile_on[2], row_ok[2][2];
 #pragma unroll
-  for (int q = 0; q < NP / 2; ++q) acc[q] = 0.f;
+  for (int s = 0; s < 2; ++s) {
+    const int t = blockIdx.x * kWgradTiles + wg * 2 + s;
+    tile_on[s] = t * p.fields_per_tile < F;                         // warpgroup-uniform
+    field[s] = t * p.fields_per_tile + upper;
+    row_ok[s][0] = field[s] < F && jw < H;
+    row_ok[s][1] = field[s] < F && jw + 8 < H;
+    if (field[s] >= F) field[s] = 0;                                 // keeps the x0 reads in range
+  }
   const int64_t n_blocks = (p.BD + kWgRows - 1) / kWgRows;
   const int64_t blk0 = (int64_t)blockIdx.y * p.blocks_per_split;
   int64_t blk1 = blk0 + p.blocks_per_split;
   if (blk1 > n_blocks) blk1 = n_blocks;
-  for (int64_t blk = blk0; blk < blk1; ++blk) {
+
+  if (tid == 0) {
+    tc::mbar_init(&full[0], 1);
+    tc::mbar_init(&full[1], 1);
+    tc::fence_barrier_init();
+  }
+  __syncthreads();
+  // warp 0 brings block blk into stage st: its dC image, its x0 rows and (k >= 1) its h rows
+  auto issue = [&](int64_t blk, int st) {
     const int64_t gm0 = blk * kWgRows;
-    __syncthreads();                                       // the previous block's MMAs and reads are done
-    for (int e = tid; e < kWgRows * p.H; e += 128) {
-      const int m = e / p.H, j = e - m * p.H;
-      hs[m][j] = gm0 + m < p.BD ? p.h[(gm0 + m) * p.ldh + j] : 0.f;
+    const int rows = p.BD - gm0 < kWgRows ? (int)(p.BD - gm0) : kWgRows;      // a multiple of 4: D divides 64
+    uint8_t* sb = smem + st * lay.stage;
+    if (lane == 0) {
+      uint32_t bytes = cin_wg_dc_block_bytes(NP) + rows * F * 4;
+      if (p.h) bytes += rows * (p.hrow_bytes ? p.hrow_bytes : p.ldh * 4);
+      tc::mbar_arrive_expect_tx(&full[st], bytes);
+      tc::bulk_g2s(sb, p.dc + blk * cin_wg_dc_block_bytes(NP), cin_wg_dc_block_bytes(NP), &full[st]);
+      tc::bulk_g2s(sb + lay.x0_off, p.x0t + gm0 * F, rows * F * 4, &full[st]);
+      if (p.h && !p.hrow_bytes) tc::bulk_g2s(sb + lay.h_off, p.h + gm0 * p.ldh, rows * p.ldh * 4, &full[st]);
     }
-    if (tid < kWgRows) xs[tid] = gm0 + tid < p.BD ? p.x0t[(gm0 + tid) * p.F + i] : 0.f;
-    for (int e = tid; e < kWgRows * NP; e += 128) {
-      const int m = e / NP, l = e - m * NP;
-      const float v = (gm0 + m < p.BD && l < p.L) ? p.dc[(gm0 + m) * p.L + l] : 0.f;
-      if (do_bias && v != 0.f) atomicAdd(&bsum[l], v);
-      const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-      const int off = ((m >> 3) * (NP >> 3) + (l >> 3)) * 128 + (l & 7) * 16 + (m & 7) * 2;
-      *reinterpret_cast<__nv_bfloat16*>(bimg + off) = hi;
-      *reinterpret_cast<__nv_bfloat16*>(bimg + img + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
+    if (p.h && p.hrow_bytes) {
+      __syncwarp();
+      for (int r = lane; r < rows; r += 32)
+        tc::bulk_g2s(sb + lay.h_off + r * p.hpitch * 4, p.h + (gm0 + r) * p.ldh, p.hrow_bytes, &full[st]);
     }
-    tc::fence_proxy_async_smem();
-    __syncthreads();
-    const uint32_t b_hi = tc::smem_u32(bimg), b_lo = b_hi + img;
-    uint32_t ahi[kWgRows / 16][4], alo[kWgRows / 16][4];
+  };
+  if (warp == 0 && blk0 < blk1) issue(blk0, 0);
+
+  float acc[2][NP / 2];
 #pragma unroll
-    for (int ks = 0; ks < kWgRows / 16; ++ks) {
+  for (int s = 0; s < 2; ++s)
 #pragma unroll
-      for (int f = 0; f < 4; ++f) {
-        const int j = j0 + ((f & 1) << 3), m = ks * 16 + ((f >> 1) << 3) + c2;
-        const float z0 = j < p.H ? xs[m] * hs[m][j] : 0.f, z1 = j < p.H ? xs[m + 1] * hs[m + 1][j] : 0.f;
-        tc::split_bf16x2(z0, z1, ahi[ks][f], alo[ks][f]);
+    for (int q = 0; q < NP / 2; ++q) acc[s][q] = 0.f;
+  uint32_t n = 0;
+  for (int64_t blk = blk0; blk < blk1; ++blk, ++n) {
+    const int st = n & 1;
+    // the other stage was released by the __syncthreads that ended the previous block
+    if (warp == 0 && blk + 1 < blk1) issue(blk + 1, st ^ 1);
+    const int rows = p.BD - blk * kWgRows < kWgRows ? (int)(p.BD - blk * kWgRows) : kWgRows;
+    const uint8_t* sb = smem + st * lay.stage;
+    const float* xs = reinterpret_cast<const float*>(sb + lay.x0_off);          // [m][i]
+    const float* hs = p.h ? reinterpret_cast<const float*>(sb + lay.h_off) : xs; // [m][j], pitch hp
+    const int hp = p.h ? p.hpitch : F;
+    const uint32_t b_hi = tc::smem_u32(sb), b_lo = b_hi + img;
+    tc::mbar_wait(&full[st], (n >> 1) & 1);
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      if (!tile_on[s]) continue;
+      uint32_t ahi[kWgRows / 16][4], alo[kWgRows / 16][4];
+#pragma unroll
+      for (int ks = 0; ks < kWgRows / 16; ++ks) {
+#pragma unroll
+        for (int f = 0; f < 4; ++f) {
+          const int r = f & 1, j = jw + 8 * r, m = ks * 16 + ((f >> 1) << 3) + c2;
+          const bool ok = row_ok[s][r];
+          const float z0 = ok && m < rows ? xs[m * F + field[s]] * hs[m * hp + j] : 0.f;
+          const float z1 = ok && m + 1 < rows ? xs[(m + 1) * F + field[s]] * hs[(m + 1) * hp + j] : 0.f;
+          tc::split_bf16x2(z0, z1, ahi[ks][f], alo[ks][f]);
+        }
       }
-    }
-    tc::wgmma_fence();
+      tc::wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < kWgRows / 16; ++ks) {
-      const uint64_t dhi = tc::make_smem_desc(b_hi + ks * 2 * lbo_b, lbo_b, 128);
-      tc::Wgmma<NP>::rs(acc, ahi[ks], dhi, 1u);
-      tc::Wgmma<NP>::rs(acc, alo[ks], dhi, 1u);
-      tc::Wgmma<NP>::rs(acc, ahi[ks], tc::make_smem_desc(b_lo + ks * 2 * lbo_b, lbo_b, 128), 1u);
+      for (int ks = 0; ks < kWgRows / 16; ++ks) {
+        const uint64_t dhi = tc::make_smem_desc(b_hi + ks * 2 * lbo_b, lbo_b, 128);
+        tc::Wgmma<NP>::rs(acc[s], ahi[ks], dhi, 1u);
+        tc::Wgmma<NP>::rs(acc[s], alo[ks], dhi, 1u);
+        tc::Wgmma<NP>::rs(acc[s], ahi[ks], tc::make_smem_desc(b_lo + ks * 2 * lbo_b, lbo_b, 128), 1u);
+      }
+      tc::wgmma_commit();
     }
-    tc::wgmma_commit();
     tc::wgmma_wait<0>();
-    tc::wgmma_fence_acc(acc);
+    tc::wgmma_fence_acc(acc[0]);
+    tc::wgmma_fence_acc(acc[1]);
+    __syncthreads();
   }
 #pragma unroll
-  for (int q = 0; q < NP / 2; ++q) {
-    const int j = j0 + (((q >> 1) & 1) << 3), l = 8 * (q >> 2) + c2 + (q & 1);
-    if (j < p.H && l < p.L && acc[q] != 0.f) atomicAdd(p.dw + ((int64_t)i * p.H + j) * p.L + l, acc[q]);
-  }
-  if (do_bias) {
-    __syncthreads();
-    for (int l = tid; l < p.L; l += 128)
-      if (bsum[l] != 0.f) atomicAdd(p.dbias + l, bsum[l]);
+  for (int s = 0; s < 2; ++s) {
+    if (!tile_on[s]) continue;
+#pragma unroll
+    for (int q = 0; q < NP / 2; ++q) {
+      const int r = (q >> 1) & 1, j = jw + 8 * r, l = 8 * (q >> 2) + c2 + (q & 1);
+      if (row_ok[s][r] && l < p.L && acc[s][q] != 0.f)
+        atomicAdd(p.dw + ((int64_t)field[s] * H + j) * p.L + l, acc[s][q]);
+    }
   }
 }
 
@@ -676,10 +789,13 @@ static size_t cin_wg_pack_t_bytes(const CinShape& s) {
   for (int k = 0; k < s.n_layers; ++k) b += (size_t)s.F * cin_wg_npj(s) * round_up16(s.L[k]) * 4;
   return (b + 255) / 256 * 256;
 }
-size_t cin_wg_bwd_workspace_bytes(const CinShape& s, int B) {
-  return cin_wg_pack_t_bytes(s) + (size_t)B * s.D * s.sumL * sizeof(float);
+// dC_k images of every layer: whole 64-row blocks of cin_wg_np columns (4 bytes per element, hi + lo)
+static size_t cin_wg_dc_layer_bytes(const CinShape& s, int B) {
+  return (size_t)(((int64_t)B * s.D + kWgRows - 1) / kWgRows) * cin_wg_dc_block_bytes(cin_wg_np(s));
 }
-static int wgrad_smem_bytes(int NP) { return 2 * NP * kWgRows * 2 + kWgRows * (kWgMaxHp + 1) * 4 + kWgRows * 4 + NP * 4; }
+size_t cin_wg_bwd_workspace_bytes(const CinShape& s, int B) {
+  return cin_wg_pack_t_bytes(s) + s.n_layers * cin_wg_dc_layer_bytes(s, B);
+}
 
 template <int NPJ>
 static int cin_wg_dgrad_launch(const CinWgBwdParams& p, cudaStream_t st) {
@@ -696,10 +812,10 @@ static int cin_wg_dgrad_launch(const CinWgBwdParams& p, cudaStream_t st) {
 }
 
 template <int NP>
-static int cin_wg_wgrad_launch(const CinWgWgradParams& p, int n_splits, cudaStream_t st) {
-  const int smem = wgrad_smem_bytes(NP);
+static int cin_wg_wgrad_launch(const CinWgWgradParams& p, int n_groups, int n_splits, cudaStream_t st) {
+  const int smem = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0).total;
   DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_wgrad_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  cin_wg_wgrad_kernel<NP><<<dim3(p.F, n_splits), 128, smem, st>>>(p);
+  cin_wg_wgrad_kernel<NP><<<dim3(n_groups, n_splits), 256, smem, st>>>(p);
   DTB_LAUNCH_OK();
   return DTB_OK;
 }
@@ -712,28 +828,27 @@ int cin_wg_bwd(const CinShape& s, const int32_t* idx, const int64_t* row_offsets
     return DTB_ERR_INVALID_ARG;
   }
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-  float* dc = reinterpret_cast<float*>(ws + cin_wg_pack_t_bytes(s));
+  uint8_t* dc = ws + cin_wg_pack_t_bytes(s);
   const float* sv = reinterpret_cast<const float*>(saved);
-  const int npj = cin_wg_npj(s);
+  const int npj = cin_wg_npj(s), np = cin_wg_np(s);
   size_t dc_off[kCinMaxLayers], saved_off[kCinMaxLayers];
   {
-    size_t d = 0, o = (size_t)B * s.D * s.F;
+    size_t o = (size_t)B * s.D * s.F;
     for (int k = 0; k < s.n_layers; ++k) {
-      dc_off[k] = d; saved_off[k] = o;
-      d += (size_t)B * s.D * s.L[k];
+      dc_off[k] = k * cin_wg_dc_layer_bytes(s, B); saved_off[k] = o;
       o += (size_t)B * s.D * s.L[k];
     }
   }
   if (phase != 2) {
     CinWgBwdParams p{};
     p.idx = idx; p.row_offsets = row_offsets; p.wpack = ws; p.d_pooled = d_pooled; p.saved = sv;
-    p.grad_table = grad_table; p.dc = dc;
-    p.B = B; p.D = s.D; p.F = s.F; p.n_layers = s.n_layers; p.act = act; p.P = s.P;
+    p.grad_table = grad_table; p.dc = dc; p.dbias = d_bias;
+    p.B = B; p.D = s.D; p.F = s.F; p.n_layers = s.n_layers; p.act = act; p.P = s.P; p.NPdc = np;
     size_t woff = 0;
     for (int k = 0; k < s.n_layers; ++k) {
       p.L[k] = s.L[k]; p.LP[k] = round_up16(s.L[k]); p.H[k] = s.H[k]; p.hid_n[k] = k + 1 < s.n_layers ? s.H[k + 1] : 0;
       p.pool_lo[k] = s.pool_lo[k]; p.pool_n[k] = s.pool_n[k]; p.pcol0[k] = s.pcol0[k];
-      p.wpack_off[k] = woff; p.saved_off[k] = saved_off[k]; p.dc_off[k] = dc_off[k];
+      p.wpack_off[k] = woff; p.saved_off[k] = saved_off[k]; p.dc_off[k] = dc_off[k]; p.bias_off[k] = s.b_off[k];
       const int64_t total = (int64_t)s.F * npj * p.LP[k];
       int blocks = (int)((total + 255) / 256);
       if (blocks > sm_count() * 8) blocks = sm_count() * 8;
@@ -750,25 +865,37 @@ int cin_wg_bwd(const CinShape& s, const int32_t* idx, const int64_t* row_offsets
     if (rc != DTB_OK) return rc;
   }
   if (phase != 1) {
-    const int np = cin_wg_np(s);
     const int64_t BD = (int64_t)B * s.D;
     const int64_t n_blocks = (BD + kWgRows - 1) / kWgRows;
     for (int k = 0; k < s.n_layers; ++k) {
       CinWgWgradParams w{};
-      w.x0t = sv; w.h = k == 0 ? sv : sv + saved_off[k - 1]; w.ldh = k == 0 ? s.F : s.L[k - 1];
-      w.dc = dc + dc_off[k]; w.dw = d_weights + s.w_off[k]; w.dbias = d_bias ? d_bias + s.b_off[k] : nullptr;
+      w.x0t = sv; w.h = k == 0 ? nullptr : sv + saved_off[k - 1]; w.ldh = k == 0 ? s.F : s.L[k - 1];
+      w.dc = dc + dc_off[k]; w.dw = d_weights + s.w_off[k];
       w.BD = BD; w.F = s.F; w.H = s.H[k]; w.L = s.L[k];
-      int64_t splits = (int64_t)sm_count() * 2 / s.F;
+      w.fields_per_tile = s.H[k] <= 32 ? 2 : 1;
+      // rows of T_{k-1} start 16-byte aligned when ldh % 4 == 0: copy only their first H columns, to a pitch that makes
+      // the A-fragment reads free of bank conflicts (pitch % 16 in {4, 12}); otherwise copy the whole block
+      if (k > 0 && w.ldh % 4 == 0) {
+        const int h4 = (s.H[k] + 3) / 4 * 4;
+        w.hrow_bytes = h4 * 4;
+        w.hpitch = h4 + (20 - h4 % 16) % 16;
+      } else {
+        w.hrow_bytes = 0;
+        w.hpitch = w.ldh;
+      }
+      const int a_tiles = (s.F + w.fields_per_tile - 1) / w.fields_per_tile;
+      const int groups = (a_tiles + kWgradTiles - 1) / kWgradTiles;
+      int64_t splits = (int64_t)sm_count() / groups;
       if (splits < 1) splits = 1;
       if (splits > n_blocks) splits = n_blocks;
       w.blocks_per_split = (int)((n_blocks + splits - 1) / splits);
       splits = (n_blocks + w.blocks_per_split - 1) / w.blocks_per_split;
       int rc;
       switch (np) {
-        case 16: rc = cin_wg_wgrad_launch<16>(w, (int)splits, st); break;
-        case 32: rc = cin_wg_wgrad_launch<32>(w, (int)splits, st); break;
-        case 64: rc = cin_wg_wgrad_launch<64>(w, (int)splits, st); break;
-        default: rc = cin_wg_wgrad_launch<128>(w, (int)splits, st); break;
+        case 16: rc = cin_wg_wgrad_launch<16>(w, groups, (int)splits, st); break;
+        case 32: rc = cin_wg_wgrad_launch<32>(w, groups, (int)splits, st); break;
+        case 64: rc = cin_wg_wgrad_launch<64>(w, groups, (int)splits, st); break;
+        default: rc = cin_wg_wgrad_launch<128>(w, groups, (int)splits, st); break;
       }
       if (rc != DTB_OK) return rc;
     }
