@@ -1060,6 +1060,10 @@ int dtb_pnn_bwd(const int32_t* idx, const float* table, const int64_t* row_offse
   DTB_CHECK_ARG(!d_op || (op_kernel && d_op_kernel), "outer product gradient without kernel buffers");
   if (B == 0 || (!d_ip && !d_op)) return DTB_OK;
   const int P = F * (F - 1) / 2;
+  if (P > 1024) {        // the forward's limit: the generic kernels below run one thread per pair
+    set_error("dtb_pnn_bwd: %d pairs exceed one CTA", P);
+    return DTB_ERR_UNSUPPORTED;
+  }
   const int threads = (P + 31) / 32 * 32;
   cudaStream_t st = (cudaStream_t)stream;
   const size_t per = kernel_type == 0 ? (size_t)D * D : (kernel_type == 1 ? (size_t)D : 1);

@@ -251,7 +251,8 @@ int dtb_cross_bwd(const float* X, const float* kernels, const float* biases, con
 
 /* ---- InnerProduct / OuterProduct (layers.py:473-487, 541-581), gather fused --------------- */
 /* ip[B,P] (NULL: skipped), op[B,P] (NULL: skipped); P = F(F-1)/2 pairs (i<j) row-major.
- * kernel_type 0 mat [D,P,D], 1 vec [P,D], 2 num [P,1]. */
+ * kernel_type 0 mat [D,P,D], 1 vec [P,D], 2 num [P,1].  Both refuse P > 1024 (F >= 46) with
+ * DTB_ERR_UNSUPPORTED. */
 int dtb_pnn_fwd(const int32_t* idx, const float* table, const int64_t* row_offsets,
                 const float* op_kernel, float* ip, float* op, int B, int F, int D, int kernel_type,
                 int* status, void* stream);

@@ -61,6 +61,12 @@ SHAPES = [  # (vocab sizes, D, C, B)
     ([11, 3], 2, 0, 33),          # D=2: generic (non-vector) path, no continuous
     ([13], 8, 2, 19),             # single categorical column
     ([6, 7, 8], 32, 1, 40),       # D=32
+    ([30] * 26, 32, 13, 77),      # F*D/4 = 208: fm_linear_fwd_vec<2>
+    ([20] * 39, 16, 5, 50),       # 39 fields at D=16 (156 slots): fm_linear_fwd_vec<2>
+    ([30] * 26, 64, 4, 45),       # 416 slots: fm_linear_fwd_vec_loop; the backward reduces over Q = 16 lanes
+    ([10] * 26, 128, 0, 19),      # 832 slots: fm_linear_fwd_vec_loop, Q = 32; no continuous
+    ([7, 9, 5], 10, 2, 31),       # D % 4 != 0: generic path
+    ([7, 9, 5, 6], 12, 3, 21),    # D = 12, Q = 3 not a power of two: generic path
 ]
 
 
@@ -201,7 +207,10 @@ def test_concat_and_batchnorm(nat, vocab, d, c, b):
 # row counts / odd widths, more than one 256-column output tile (dX of the 1079-wide layer), K smaller than one chunk
 @pytest.mark.parametrize('rows,i,o,act', [(300, 429, 128, 1), (300, 128, 64, 1), (77, 64, 1, 0), (50, 1, 1, 0),
                                            (64, 37, 3, 0), (5, 10, 20, 1), (1000, 1079, 128, 1), (2600, 32, 128, 1),
-                                           (129, 845, 128, 0), (33, 7, 300, 1), (4097, 64, 64, 0)])
+                                           (129, 845, 128, 0), (33, 7, 300, 1), (4097, 64, 64, 0),
+                                           # out_dim 9..16: the N = 16 GEMMs with the bias / relu epilogue and the
+                                           # N = 16 weight gradient; odd widths: unpaired stores of Y (and of dX)
+                                           (300, 64, 10, 1), (130, 50, 16, 0), (257, 37, 33, 1)])
 def test_dense_fwd_bwd(nat, rows, i, o, act):
     g = np.random.default_rng(7)
     x = g.normal(size=(rows, i)).astype(np.float32)
@@ -687,7 +696,10 @@ def test_cin_tensor_core_backward(nat, f, d, sizes, direct, use_bias, act, b):
 # ---------------------------------------------------------------------------------------------
 # PNN products and the AutoInt attention core
 # ---------------------------------------------------------------------------------------------
-@pytest.mark.parametrize('f,d,b', [(26, 16, 70), (5, 4, 33), (2, 8, 9), (7, 3, 20), (6, 32, 150), (26, 16, 300), (12, 8, 200)])
+# (26, 32, 40): the kernel-gradient kernel halves its row tile to 16; (45, 4, 9): the last field count both directions
+# accept (990 pairs)
+@pytest.mark.parametrize('f,d,b', [(26, 16, 70), (5, 4, 33), (2, 8, 9), (7, 3, 20), (6, 32, 150), (26, 16, 300), (12, 8, 200),
+                                   (26, 32, 40), (45, 4, 9)])
 @pytest.mark.parametrize('ktype', ['mat', 'vec', 'num'])
 def test_pnn_fwd_bwd(nat, f, d, b, ktype):
     vocab = [11 + i for i in range(f)]
@@ -723,8 +735,11 @@ def test_pnn_fwd_bwd(nat, f, d, b, ktype):
     np.testing.assert_allclose(dk.cpu().numpy(), grads[-1].numpy(), rtol=1e-3, atol=1e-4 * np.abs(grads[-1].numpy()).max())
 
 
+# F = 98 / 99: 4 / 2 rows per CTA at D = H = 16 (shared memory); 135 / 136: 2 / 1; 178: the last field count accepted
 @pytest.mark.parametrize('f,d,h,b,act', [(26, 16, 16, 70, 'relu'), (5, 4, 5, 33, 'linear'), (3, 8, 32, 200, 'relu'),
-                                         (7, 32, 8, 20, 'relu'), (2, 16, 4, 9, 'relu'), (12, 8, 16, 300, 'relu')])
+                                         (7, 32, 8, 20, 'relu'), (2, 16, 4, 9, 'relu'), (12, 8, 16, 300, 'relu'),
+                                         (98, 16, 16, 17, 'relu'), (99, 16, 16, 9, 'relu'), (135, 16, 16, 10, 'relu'),
+                                         (136, 16, 16, 11, 'relu'), (178, 16, 16, 9, 'relu')])
 def test_afm_fwd_bwd(nat, f, d, h, b, act):
     """AFM attention pooling (layers.py:790-804) and its gradients against the fp64 oracle's autograd."""
     vocab = [11 + i for i in range(f)]
@@ -762,7 +777,9 @@ def test_afm_fwd_bwd(nat, f, d, h, b, act):
         np.testing.assert_allclose(got.cpu().numpy(), ref, rtol=2e-3, atol=2e-4 * max(np.abs(ref).max(), scale), err_msg=name)
 
 
-@pytest.mark.parametrize('f,d,b', [(26, 16, 150), (5, 4, 33), (2, 8, 9), (7, 32, 130), (12, 8, 300)])
+# D = 32: the weight-gradient row tile halves to 16 at 26 fields and to 8 at 51, the last field count accepted
+@pytest.mark.parametrize('f,d,b', [(26, 16, 150), (5, 4, 33), (2, 8, 9), (7, 32, 130), (12, 8, 300), (26, 32, 70),
+                                   (51, 32, 9)])
 @pytest.mark.parametrize('bt', ['field_all', 'field_each', 'field_interaction'])
 def test_bilinear_fwd_bwd(nat, f, d, b, bt):
     """BilinearInteraction (layers.py:358-372) on a dense block and its gradients against the fp64 oracle's autograd."""
@@ -857,7 +874,7 @@ def test_fgcnn_conv_and_pool_fwd_bwd(nat, b, h, w, cin, cout, kh, pool, act):
 def test_dense_tanh_activation(nat):
     """DTB_ACT_TANH in the Dense epilogues (wide: wgmma path, narrow: row-dot path) and its backward."""
     g = np.random.default_rng(82)
-    for rows, i, o in ((300, 36, 40), (200, 48, 5)):
+    for rows, i, o in ((300, 36, 40), (200, 48, 5), (129, 40, 10), (70, 24, 45)):
         x = g.normal(size=(rows, i)).astype(np.float32)
         w = (g.normal(size=(i, o)) / np.sqrt(i)).astype(np.float32)
         bias = (g.normal(size=(o,)) * 0.1).astype(np.float32)
@@ -908,8 +925,14 @@ def test_senet_pool_and_scale(nat, op):
     np.testing.assert_allclose(da.cpu().numpy(), wa.numpy(), rtol=1e-4, atol=1e-5)
 
 
+# generic kernels: D % 4 != 0 (D = 10), head width 12, heads * F = 312 > 256, heads * F = 1024 (the largest accepted);
+# (5, 150, 64, 1): one row of the backward needs more than 220 KiB, the forward still fits; head widths 32 and 2 and the
+# widest accepted head (64, two heads)
 @pytest.mark.parametrize('b,f,d,heads,res', [(40, 26, 32, 4, True), (17, 5, 4, 1, True), (9, 7, 16, 2, False), (3, 1, 8, 8, True),
-                                               (1001, 26, 16, 1, True), (131, 26, 32, 4, False), (70, 3, 64, 1, True)])
+                                               (1001, 26, 16, 1, True), (131, 26, 32, 4, False), (70, 3, 64, 1, True),
+                                               (13, 5, 10, 2, True), (21, 6, 24, 2, False), (9, 39, 16, 8, True),
+                                               (2, 128, 64, 8, True), (5, 150, 64, 1, True), (33, 26, 32, 1, True),
+                                               (19, 13, 16, 8, False), (7, 5, 128, 2, True)])
 def test_attention_core_fwd_bwd(nat, b, f, d, heads, res):
     g = np.random.default_rng(54)
     qkvr = np.maximum(g.normal(size=(b, f, 4 * d)), 0).astype(np.float32)       # relu outputs
