@@ -24,6 +24,16 @@ lib = ctypes.CDLL(LIB_PATH)
 P = c_void_p   # every device pointer travels as void*
 _IP = POINTER(c_int)
 
+
+class OptimParams(ctypes.Structure):
+    """``dtb_optim_params`` (host memory, read at call time): hyperparameters of SGD / RMSprop / Adagrad."""
+    _fields_ = [('kind', c_int), ('flag', c_int), ('lr', c_float), ('momentum', c_float), ('rho', c_double),
+                ('eps', c_float)]
+
+
+OPTIM_SGD, OPTIM_RMSPROP, OPTIM_ADAGRAD = 1, 2, 3
+_OPP = POINTER(OptimParams)
+
 _SIGNATURES = {
     'dtb_version': (c_int, []),
     'dtb_last_error': (c_char_p, []),
@@ -56,6 +66,13 @@ _SIGNATURES = {
     'dtb_adam_rows_apply_dev': (c_int, [P, P, P, P, P, P, P, P, P, c_double, c_double, c_float, c_int, c_int, c_int, P]),
     'dtb_step_increment': (c_int, [P, P]),
     'dtb_adam_rows_flush': (c_int, [P, P, P, P, P, c_int, c_double, c_double, c_float, c_int64, c_int, P]),
+    'dtb_optim_dense': (c_int, [P, P, P, P, P, c_int64, _OPP, c_int, P]),
+    'dtb_optim_rows_catchup': (c_int, [P, P, P, P, P, P, P, c_int, _OPP, c_int, c_int, c_int, P]),
+    'dtb_optim_rows_apply': (c_int, [P, P, P, P, P, P, P, P, c_int, _OPP, c_int, c_int, c_int, P]),
+    'dtb_optim_rows_flush': (c_int, [P, P, P, P, P, c_int, _OPP, c_int64, c_int, P]),
+    'dtb_optim_rows_catchup_dev': (c_int, [P, P, P, P, P, P, P, P, _OPP, c_int, c_int, c_int, P]),
+    'dtb_optim_rows_apply_dev': (c_int, [P, P, P, P, P, P, P, P, P, _OPP, c_int, c_int, c_int, P]),
+    'dtb_optim_rows_flush_dev': (c_int, [P, P, P, P, P, P, _OPP, c_int64, c_int, P]),
     'dtb_grad_rows_pack': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),

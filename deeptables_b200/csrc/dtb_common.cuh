@@ -91,4 +91,44 @@ __device__ __forceinline__ void adam_update(float& p, float& m, float& v, float 
   p = __fsub_rn(p, __fdiv_rn(__fmul_rn(m, alpha), __fadd_rn(__fsqrt_rn(v), eps)));
 }
 
+// keras.optimizers.SGD.update_step, Keras's operation order, every rounding pinned (optim.cu):
+//   momentum = 0 : p -= g*lr
+//   otherwise    : m = m*mu - g*lr ; p += m   (nesterov: p += m*mu - g*lr)
+__device__ __forceinline__ void sgd_update(float& p, float& m, float g, float lr, float mu, bool nesterov) {
+  const float glr = __fmul_rn(g, lr);
+  if (mu == 0.f) {
+    p = __fsub_rn(p, glr);
+    return;
+  }
+  m = __fsub_rn(__fmul_rn(m, mu), glr);
+  p = __fadd_rn(p, nesterov ? __fsub_rn(__fmul_rn(m, mu), glr) : m);
+}
+
+// keras.optimizers.RMSprop.update_step: v = rho*v + (1-rho)*g^2 ; centered: a = rho*a + (1-rho)*g, den = v - a^2 + eps,
+// else den = v + eps ; inc = lr*g / sqrt(den) ; momentum > 0: mom = mu*mom + inc, p -= mom ; else p -= inc
+__device__ __forceinline__ void rmsprop_update(float& p, float& v, float& a, float& mom, float g, float lr, float rho,
+                                               float omr, float mu, float eps, bool centered) {
+  v = __fadd_rn(__fmul_rn(rho, v), __fmul_rn(omr, __fmul_rn(g, g)));
+  float den;
+  if (centered) {
+    a = __fadd_rn(__fmul_rn(rho, a), __fmul_rn(omr, g));
+    den = __fadd_rn(__fsub_rn(v, __fmul_rn(a, a)), eps);
+  } else {
+    den = __fadd_rn(v, eps);
+  }
+  const float inc = __fdiv_rn(__fmul_rn(lr, g), __fsqrt_rn(den));
+  if (mu > 0.f) {
+    mom = __fadd_rn(__fmul_rn(mu, mom), inc);
+    p = __fsub_rn(p, mom);
+  } else {
+    p = __fsub_rn(p, inc);
+  }
+}
+
+// keras.optimizers.Adagrad.update_step: acc += g^2 ; p -= lr*g / sqrt(acc + eps)
+__device__ __forceinline__ void adagrad_update(float& p, float& acc, float g, float lr, float eps) {
+  acc = __fadd_rn(acc, __fmul_rn(g, g));
+  p = __fsub_rn(p, __fdiv_rn(__fmul_rn(lr, g), __fsqrt_rn(__fadd_rn(acc, eps))));
+}
+
 }  // namespace dtb

@@ -4,7 +4,8 @@ Same constructor and public methods (fit / predict / evaluate / apply / save / r
 ``model``, ``model_desc``, ``config``), same graph (``__build_model``, reference deepmodel.py:259-317:
 inputs -> MultiColumnEmbedding -> flatten/concat + BatchNormalization -> net builders -> stacking ->
 ``task_output``), same training contract (Adam(1e-3) + BCE/MSE/CCE when ``optimizer``/``loss`` are
-'auto', reference deepmodel.py:319-346; ``steps_per_epoch`` / ``validation_steps`` arithmetic,
+'auto', reference deepmodel.py:319-346; SGD / RMSprop / Adagrad / Adam at other hyperparameters through
+``optimizers.py``; ``steps_per_epoch`` / ``validation_steps`` arithmetic,
 reference deepmodel.py:76-83).  The numerics run in hand-written sm_90a kernels behind the C ABI;
 torch supplies device memory and the autograd tape only.
 
@@ -23,7 +24,7 @@ from typing import Union
 import numpy as np
 import torch
 
-from . import consts, deepnets, dp, engine as E, layers as L
+from . import consts, deepnets, dp, engine as E, layers as L, optimizers as O
 from ._native import ptr, check, stream_ptr
 from . import _native as N
 
@@ -127,14 +128,20 @@ class _Scope:
         return mat.reshape(mat.shape[0], -1)
 
     # ---- flat storage so Adam and the DP all-reduce are one launch / one bucket -------------------
-    def freeze(self):
+    def freeze(self, slot_inits=None):
+        """slot_inits: initial values of the SGD / RMSprop / Adagrad state slots (optimizers.slot_inits); None = Adam's
+        flat_m, flat_v."""
         names = list(self.params)
         sizes = [self.params[n].numel() for n in names]
         total = sum(sizes)
         self.flat_p = torch.empty(total, dtype=torch.float32, device=self.device)
         self.flat_g = torch.zeros(total, dtype=torch.float32, device=self.device)
-        self.flat_m = torch.zeros(total, dtype=torch.float32, device=self.device)
-        self.flat_v = torch.zeros(total, dtype=torch.float32, device=self.device)
+        if slot_inits is None:
+            self.flat_m = torch.zeros(total, dtype=torch.float32, device=self.device)
+            self.flat_v = torch.zeros(total, dtype=torch.float32, device=self.device)
+        else:
+            self.flat_slots = [None if s is None else torch.full((total,), s, dtype=torch.float32, device=self.device)
+                               for s in slot_inits]
         off = 0
         for n, sz in zip(names, sizes):
             old = self.params[n]
@@ -257,6 +264,8 @@ class DeepModel:
         self._focal = None                  # (gamma, alpha) when ModelConfig.loss is one of the focal losses
         self._alpha = None
         self._step_dev = None              # optimiser step counter in device memory (CUDA-graph replay of the train step)
+        self._opt = None                   # optimizers.OptimizerSpec resolved from ModelConfig.optimizer
+        self._opt_native = None            # its dtb_optim_params (SGD / RMSprop / Adagrad)
         self._graphs = {}
         self._graph_failed = False
         if model_file is not None:
@@ -267,8 +276,9 @@ class DeepModel:
     # ------------------------------------------------------------------------------------------
     def _build_model(self):
         cfg = self.config
-        if cfg.optimizer != 'auto':
-            raise NotImplementedError("only optimizer='auto' (Adam 1e-3) is built natively")
+        self._opt = O.resolve(cfg.optimizer)
+        self._opt_native = None if self._opt.kind == 'adam' else _native_optim_params(self._opt)
+        slot_inits = None if self._opt.kind == 'adam' else O.slot_inits(self._opt)
         self._focal = None
         if isinstance(cfg.loss, L.CategoricalFocalLoss):
             if self.task != consts.TASK_MULTICLASS:
@@ -288,6 +298,7 @@ class DeepModel:
         if self.n_fields:
             self.table = E.EmbeddingTable([c.vocabulary_size for c in self.categorical_columns], self.emb_dim,
                                           self.device, cfg.embeddings_initializer, self._scope.generator)
+            self.table.slot_inits = slot_inits
         self.model_desc = ModelDesc()
         if self.n_fields:
             self.model_desc.add_input('all_categorical_vars', self.n_fields)
@@ -298,7 +309,7 @@ class DeepModel:
         self.model_desc.set_dense(cfg.dense_dropout, False)
         self.model_desc.nets = cfg.nets
         self.model_desc.stacking = cfg.stacking_op
-        self.model_desc.optimizer = 'Adam'
+        self.model_desc.optimizer = self._opt.keras_name
         self.model_desc.loss = {consts.TASK_BINARY: 'binary_crossentropy', consts.TASK_MULTILABEL:
                                 'binary_crossentropy', consts.TASK_REGRESSION: 'mse'}.get(
             self.task, 'binary_crossentropy' if self.num_classes == 2 else 'categorical_crossentropy')
@@ -309,7 +320,7 @@ class DeepModel:
         cont = torch.zeros(2, self.n_cont, dtype=torch.float32, device=self.device) if self.n_cont else None
         with torch.no_grad():
             self._forward(cat, cont, training=False, describe=True)
-        self._scope.freeze()
+        self._scope.freeze(slot_inits)
         dp.broadcast_parameters([self._scope.flat_p, self.table.weight if self.table is not None else None])
         self._loss_acc = torch.zeros(1, dtype=torch.float64, device=self.device)
         self.model = KerasLikeModel(self)
@@ -407,7 +418,8 @@ class DeepModel:
     def _alpha_table(self, upto):
         if self._alpha is None or self._alpha.numel() <= upto:
             n = max(4096, 2 * (upto + 1))
-            vals = [0.0] + [E.adam_alpha(s) for s in range(1, n)]
+            o = self._opt
+            vals = [0.0] + [E.adam_alpha(s, o.learning_rate, o.beta_1, o.beta_2) for s in range(1, n)]
             self._alpha = torch.tensor(vals, dtype=torch.float32, device=self.device)
         return self._alpha
 
@@ -434,17 +446,29 @@ class DeepModel:
         t = self.table
         if t is None or not t.lazy_active or t.last_step is None:
             return
+        o = self._opt
+        if o.kind != 'adam':
+            s = [ptr(x) for x in t.slots]
+            if dev_step:
+                check(N.lib.dtb_optim_rows_catchup_dev(ptr(cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.last_step),
+                                                       ptr(self._step_dev), self._opt_native, cat.shape[0], t.n_fields,
+                                                       t.dim, stream_ptr()), 'optim_rows_catchup_dev')
+            elif upto > 0:
+                check(N.lib.dtb_optim_rows_catchup(ptr(cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.last_step), upto,
+                                                   self._opt_native, cat.shape[0], t.n_fields, t.dim, stream_ptr()),
+                      'optim_rows_catchup')
+            return
         if dev_step:          # CUDA-graph form: "steps done so far" is read from device memory
             check(N.lib.dtb_adam_rows_catchup_dev(ptr(cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m), ptr(t.v),
-                                                  ptr(t.last_step), ptr(self._alpha), ptr(self._step_dev), E.ADAM_B1,
-                                                  E.ADAM_B2, E.ADAM_EPS, cat.shape[0], t.n_fields, t.dim, stream_ptr()),
+                                                  ptr(t.last_step), ptr(self._alpha), ptr(self._step_dev), o.beta_1,
+                                                  o.beta_2, o.epsilon, cat.shape[0], t.n_fields, t.dim, stream_ptr()),
                   'adam_rows_catchup_dev')
             return
         if upto <= 0:
             return
         check(N.lib.dtb_adam_rows_catchup(ptr(cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m), ptr(t.v),
-                                          ptr(t.last_step), ptr(self._alpha_table(upto)), upto, E.ADAM_B1,
-                                          E.ADAM_B2, E.ADAM_EPS, cat.shape[0], t.n_fields, t.dim, stream_ptr()),
+                                          ptr(t.last_step), ptr(self._alpha_table(upto)), upto, o.beta_1,
+                                          o.beta_2, o.epsilon, cat.shape[0], t.n_fields, t.dim, stream_ptr()),
               'adam_rows_catchup')
 
     def train_step(self, cat, cont, y, sample_weight=None):
@@ -481,38 +505,66 @@ class DeepModel:
         union_cat = cat
         if self._dist:
             union_cat = self._exchange_gradients(cat)
+        o = self._opt
+        if o.kind != 'adam':
+            self._optim_step(union_cat, step, dev_step)
+            if dev_step:
+                check(N.lib.dtb_step_increment(ptr(self._step_dev), stream_ptr()), 'step_increment')
+            return prob
         if dev_step:
             check(N.lib.dtb_adam_dense_dev(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
-                                           scope.flat_p.numel(), ptr(self._alpha), ptr(self._step_dev), E.ADAM_B1,
-                                           E.ADAM_B2, E.ADAM_EPS, 1, stream_ptr()), 'adam_dense_dev')
+                                           scope.flat_p.numel(), ptr(self._alpha), ptr(self._step_dev), o.beta_1,
+                                           o.beta_2, o.epsilon, 1, stream_ptr()), 'adam_dense_dev')
             if t is not None:
                 if t.lazy_active:
                     check(N.lib.dtb_adam_rows_apply_dev(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m), ptr(t.v),
                                                         ptr(t.grad), ptr(t.last_step), ptr(self._alpha), ptr(self._step_dev),
-                                                        E.ADAM_B1, E.ADAM_B2, E.ADAM_EPS, union_cat.shape[0], t.n_fields,
+                                                        o.beta_1, o.beta_2, o.epsilon, union_cat.shape[0], t.n_fields,
                                                         t.dim, stream_ptr()), 'adam_rows_apply_dev')
                 else:
                     check(N.lib.dtb_adam_dense_dev(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(),
-                                                   ptr(self._alpha), ptr(self._step_dev), E.ADAM_B1, E.ADAM_B2, E.ADAM_EPS, 1,
+                                                   ptr(self._alpha), ptr(self._step_dev), o.beta_1, o.beta_2, o.epsilon, 1,
                                                    stream_ptr()), 'adam_dense_dev(table)')
             check(N.lib.dtb_step_increment(ptr(self._step_dev), stream_ptr()), 'step_increment')
             return prob
-        alpha = E.adam_alpha(step)
+        alpha = E.adam_alpha(step, o.learning_rate, o.beta_1, o.beta_2)
         check(N.lib.dtb_adam_dense(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
-                                   scope.flat_p.numel(), alpha, E.ADAM_B1, E.ADAM_B2, E.ADAM_EPS, 1,
+                                   scope.flat_p.numel(), alpha, o.beta_1, o.beta_2, o.epsilon, 1,
                                    stream_ptr()), 'adam_dense')
         if t is not None:
             if t.lazy_active:
                 a = self._alpha_table(step)
                 check(N.lib.dtb_adam_rows_apply(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m),
-                                                ptr(t.v), ptr(t.grad), ptr(t.last_step), ptr(a), step, E.ADAM_B1,
-                                                E.ADAM_B2, E.ADAM_EPS, union_cat.shape[0], t.n_fields, t.dim,
+                                                ptr(t.v), ptr(t.grad), ptr(t.last_step), ptr(a), step, o.beta_1,
+                                                o.beta_2, o.epsilon, union_cat.shape[0], t.n_fields, t.dim,
                                                 stream_ptr()), 'adam_rows_apply')
             else:
                 check(N.lib.dtb_adam_dense(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(),
-                                           alpha, E.ADAM_B1, E.ADAM_B2, E.ADAM_EPS, 1, stream_ptr()),
+                                           alpha, o.beta_1, o.beta_2, o.epsilon, 1, stream_ptr()),
                       'adam_dense(table)')
         return prob
+
+    def _optim_step(self, union_cat, step, dev_step):
+        """SGD / RMSprop / Adagrad step `step`: the dense sweep over the flat parameters, then the table's row-wise
+        update (lazy) or dense sweep.  Only the row form needs the step number (to count skipped steps); its
+        CUDA-graph form reads it from device memory."""
+        scope, t, hp = self._scope, self.table, self._opt_native
+        check(N.lib.dtb_optim_dense(ptr(scope.flat_p), ptr(scope.flat_g), *[ptr(x) for x in scope.flat_slots],
+                                    scope.flat_p.numel(), hp, 1, stream_ptr()), 'optim_dense')
+        if t is None:
+            return
+        s = [ptr(x) for x in t.slots]
+        if not t.lazy_active:
+            check(N.lib.dtb_optim_dense(ptr(t.weight), ptr(t.grad), *s, t.weight.numel(), hp, 1, stream_ptr()),
+                  'optim_dense(table)')
+        elif dev_step:
+            check(N.lib.dtb_optim_rows_apply_dev(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.grad),
+                                                 ptr(t.last_step), ptr(self._step_dev), hp, union_cat.shape[0], t.n_fields,
+                                                 t.dim, stream_ptr()), 'optim_rows_apply_dev')
+        else:
+            check(N.lib.dtb_optim_rows_apply(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.grad),
+                                             ptr(t.last_step), step, hp, union_cat.shape[0], t.n_fields, t.dim,
+                                             stream_ptr()), 'optim_rows_apply')
 
     # ---- CUDA-graph replay of the train step ---------------------------------------------------------------------------
     def _has_dropout(self):
@@ -538,7 +590,7 @@ class DeepModel:
                None if t is None else t.lazy_active)
         if self._step_dev is None:
             self._step_dev = torch.zeros(1, dtype=torch.int32, device=self.device)
-        if self._alpha is None or self._alpha.numel() <= self._step + 2:
+        if self._opt.kind == 'adam' and (self._alpha is None or self._alpha.numel() <= self._step + 2):
             self._graphs.clear()                       # the alpha table moves when it grows: captured pointers are stale
             self._alpha_table(self._step + 200000)
         if t is not None:
@@ -912,12 +964,17 @@ class DeepModel:
     # weights in / out, keyed by the reference's layer/weight names
     # ------------------------------------------------------------------------------------------
     def flush_optimizer_state(self):
-        """Bring every embedding row up to date (lazy Adam) -- before export / save."""
+        """Bring every embedding row up to date (lazy row-wise optimiser) -- before export / save."""
         t = self.table
         if t is not None and t.lazy_active and t.last_step is not None and self._step > 0:
+            o = self._opt
+            if o.kind != 'adam':
+                check(N.lib.dtb_optim_rows_flush(ptr(t.weight), *[ptr(x) for x in t.slots], ptr(t.last_step), self._step,
+                                                 self._opt_native, t.total_rows, t.dim, stream_ptr()), 'optim_rows_flush')
+                return
             check(N.lib.dtb_adam_rows_flush(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.last_step),
-                                            ptr(self._alpha_table(self._step)), self._step, E.ADAM_B1, E.ADAM_B2,
-                                            E.ADAM_EPS, t.total_rows, t.dim, stream_ptr()), 'adam_rows_flush')
+                                            ptr(self._alpha_table(self._step)), self._step, o.beta_1, o.beta_2,
+                                            o.epsilon, t.total_rows, t.dim, stream_ptr()), 'adam_rows_flush')
 
     def sync_replica_buffers(self):
         """Data parallel: BatchNormalization moving statistics are updated from each rank's own shard; average them
@@ -967,8 +1024,18 @@ class DeepModel:
         sd = {k: v.detach().cpu().numpy() for k, v in self.state_dict().items()}
         # optimiser state (the reference's .h5 keeps it too): Adam step, moments of the dense weights and of the
         # embedding rows (state_dict() flushed the lazy rows, so m/v are current for every row)
-        opt = {'__step__': np.array(self._step)}
-        if self._step > 0:
+        # (SGD / RMSprop / Adagrad: their state slots under __opt_slot{i}__ / __opt_table_slot{i}__); __optimizer__ names
+        # the optimiser and its hyperparameters, under which alone the state resumes
+        opt = {'__step__': np.array(self._step), '__optimizer__': np.array(self._opt.describe())}
+        if self._step > 0 and self._opt.kind != 'adam':
+            for i, s in enumerate(self._scope.flat_slots):
+                if s is not None:
+                    opt[f'__opt_slot{i}__'] = s.cpu().numpy()
+            if self.table is not None and self.table.slots is not None:
+                for i, s in enumerate(self.table.slots):
+                    if s is not None:
+                        opt[f'__opt_table_slot{i}__'] = s.cpu().numpy()
+        elif self._step > 0:
             opt['__adam_m__'] = self._scope.flat_m.cpu().numpy()
             opt['__adam_v__'] = self._scope.flat_v.cpu().numpy()
             if self.table is not None and self.table.m is not None:
@@ -988,9 +1055,31 @@ class DeepModel:
         return self.model
 
     def _restore_optimizer(self, opt):
-        """Resume Adam where the checkpoint left it; a weights-only file restarts the optimiser at step 0."""
+        """Resume the optimiser where the checkpoint left it.  A weights-only file, or one written under another optimiser
+        or other hyperparameters, restarts it at step 0.  A file without __optimizer__ was written by Adam(1e-3)."""
         step = int(opt.get('__step__', 0))
-        if step > 0 and '__adam_m__' in opt:
+        saved = str(opt['__optimizer__']) if '__optimizer__' in opt else O.resolve('auto').describe()
+        if saved != self._opt.describe():
+            step = 0
+        if step > 0 and self._opt.kind != 'adam':
+            t = self.table
+            wanted = [f'__opt_slot{i}__' for i, s in enumerate(self._scope.flat_slots) if s is not None]
+            if t is not None:
+                t.ensure_training_state()
+                wanted += [f'__opt_table_slot{i}__' for i, s in enumerate(t.slots) if s is not None]
+            if all(k in opt for k in wanted):
+                for i, s in enumerate(self._scope.flat_slots):
+                    if s is not None:
+                        s.copy_(torch.as_tensor(opt[f'__opt_slot{i}__']).to(self.device))
+                if t is not None:
+                    for i, s in enumerate(t.slots):
+                        if s is not None:
+                            s.copy_(torch.as_tensor(opt[f'__opt_table_slot{i}__']).to(self.device))
+                    t.last_step.fill_(step)
+                self._step = step
+            else:
+                self._step = 0
+        elif step > 0 and '__adam_m__' in opt:
             self._scope.flat_m.copy_(torch.as_tensor(opt['__adam_m__']).to(self.device))
             self._scope.flat_v.copy_(torch.as_tensor(opt['__adam_v__']).to(self.device))
             if self.table is not None and '__adam_table_m__' in opt:
@@ -1038,6 +1127,14 @@ class _LazyFlat:
 class _NullDesc:
     def __getattr__(self, item):
         return lambda *a, **k: None
+
+
+def _native_optim_params(spec):
+    """OptimizerSpec of SGD / RMSprop / Adagrad -> the kernels' dtb_optim_params."""
+    kind = {'sgd': N.OPTIM_SGD, 'rmsprop': N.OPTIM_RMSPROP, 'adagrad': N.OPTIM_ADAGRAD}[spec.kind]
+    flag = spec.nesterov if spec.kind == 'sgd' else spec.centered if spec.kind == 'rmsprop' else False
+    return N.OptimParams(kind=kind, flag=int(bool(flag)), lr=spec.learning_rate, momentum=spec.momentum or 0.0,
+                         rho=spec.rho or 0.0, eps=spec.epsilon or 0.0)
 
 
 def _columns(X, names):

@@ -47,6 +47,8 @@ class EmbeddingTable:
         self.grad = None
         self.m = None
         self.v = None
+        self.slot_inits = None     # SGD / RMSprop / Adagrad: initial values of state slots s0..s2 (None: Adam's m, v)
+        self.slots = None
         self.last_step = None
         self.claim = None          # per-row claim stamps of the data-parallel row exchange
         self.status = torch.zeros(1, dtype=torch.int32, device=self.device)
@@ -60,8 +62,11 @@ class EmbeddingTable:
     def ensure_training_state(self):
         if self.grad is None:
             self.grad = torch.zeros_like(self.weight)
-            self.m = torch.zeros_like(self.weight)
-            self.v = torch.zeros_like(self.weight)
+            if self.slot_inits is None:
+                self.m = torch.zeros_like(self.weight)
+                self.v = torch.zeros_like(self.weight)
+            else:
+                self.slots = [None if s is None else torch.full_like(self.weight, s) for s in self.slot_inits]
             self.last_step = torch.zeros(self.total_rows, dtype=torch.int32, device=self.device)
 
     def field_weight(self, i):

@@ -174,6 +174,50 @@ int dtb_adam_rows_apply_dev(const int32_t* idx, const int64_t* row_offsets, floa
                             double beta1, double beta2, float eps, int B, int F, int D, void* stream);
 int dtb_step_increment(int32_t* step_dev, void* stream);
 
+/* ---- keras SGD, RMSprop and Adagrad, dense semantics (optim.cu) ----------------------------------
+ * Hyperparameters travel in a host-side struct read at call time (a captured graph keeps the values
+ * of the call it captured; none of them changes during training).  State slots s0..s2 are [n] floats
+ * like p, NULL when the optimiser does not use them:
+ *   SGD     s0 = momentum buffer (when momentum > 0)
+ *   RMSprop s0 = velocity, s1 = average gradient (centered), s2 = momentum buffer (momentum > 0)
+ *   Adagrad s0 = accumulator (the caller fills it with initial_accumulator_value)
+ * The row forms follow dtb_adam_rows_*: last_step[row] = last step applied to the row, ownership per
+ * launch by atomicMax on last_step, out-of-range ids skipped, D = 4*2^k (<= 128).  Skipped
+ * zero-gradient steps are replayed in order with the same arithmetic; for SGD without momentum and
+ * for Adagrad such a step is the identity, so catch-up and flush return at once.  The `_dev` forms
+ * read the number of completed steps from device memory (CUDA-graph replay); the dense sweep does
+ * not depend on the step number, so its one form serves both. */
+#define DTB_OPTIM_SGD 1
+#define DTB_OPTIM_RMSPROP 2
+#define DTB_OPTIM_ADAGRAD 3
+typedef struct dtb_optim_params {
+  int kind;         /* DTB_OPTIM_* */
+  int flag;         /* SGD: nesterov; RMSprop: centered */
+  float lr;
+  float momentum;   /* SGD and RMSprop; 0 = no momentum slot */
+  double rho;       /* RMSprop; the kernels use rho and (float)(1.0 - rho) as Keras does */
+  float eps;        /* RMSprop and Adagrad */
+} dtb_optim_params;
+
+int dtb_optim_dense(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                    int zero_grad, void* stream);
+int dtb_optim_rows_catchup(const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1,
+                           float* s2, int32_t* last_step, int upto, const dtb_optim_params* hp, int B, int F, int D,
+                           void* stream);
+int dtb_optim_rows_apply(const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1, float* s2,
+                         float* grad_table, int32_t* last_step, int step, const dtb_optim_params* hp, int B, int F,
+                         int D, void* stream);
+int dtb_optim_rows_flush(float* table, float* s0, float* s1, float* s2, int32_t* last_step, int upto,
+                         const dtb_optim_params* hp, int64_t n_rows, int D, void* stream);
+int dtb_optim_rows_catchup_dev(const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1,
+                               float* s2, int32_t* last_step, const int32_t* step_dev, const dtb_optim_params* hp,
+                               int B, int F, int D, void* stream);
+int dtb_optim_rows_apply_dev(const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1,
+                             float* s2, float* grad_table, int32_t* last_step, const int32_t* step_dev,
+                             const dtb_optim_params* hp, int B, int F, int D, void* stream);
+int dtb_optim_rows_flush_dev(float* table, float* s0, float* s1, float* s2, int32_t* last_step,
+                             const int32_t* step_dev, const dtb_optim_params* hp, int64_t n_rows, int D, void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
