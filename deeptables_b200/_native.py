@@ -47,6 +47,8 @@ _SIGNATURES = {
     'dtb_fm_linear_bwd': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_concat_emb_dense_fwd': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P, P]),
     'dtb_concat_emb_dense_bwd': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P]),
+    'dtb_ragged_concat_emb_dense_fwd': (c_int, [P, P, P, _IP, P, P, c_int, c_int, c_int, c_int, P, P]),
+    'dtb_ragged_concat_emb_dense_bwd': (c_int, [P, P, _IP, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_batchnorm_train_fwd': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_float, c_float, P]),
     'dtb_batchnorm_infer_fwd': (c_int, [P, P, P, P, P, P, c_int, c_int, c_float, P]),
     'dtb_batchnorm_bwd': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_float, P]),

@@ -250,13 +250,9 @@ class DeepModel:
             torch.distributed.get_world_size() > 1
         self.world_size = torch.distributed.get_world_size() if self._dist else 1
         self.rank = torch.distributed.get_rank() if self._dist else 0
-        dims = {c.embeddings_output_dim for c in self.categorical_columns}
-        if len(dims) > 1:
-            raise NotImplementedError(
-                'per-column embedding widths (fixed_embedding_dim=False) are not supported by the fused '
-                f'engine yet; got {sorted(dims)}')
+        self.emb_dims = [int(c.embeddings_output_dim) for c in self.categorical_columns]
         self.n_fields = len(self.categorical_columns)
-        self.emb_dim = dims.pop() if dims else 0
+        self.emb_dim = max(self.emb_dims) if self.emb_dims else 0     # stored row width of the embedding table
         self.n_cont = sum(c.input_dim for c in self.continuous_columns)
         self._scope = None
         self.table = None
@@ -294,16 +290,24 @@ class DeepModel:
             raise NotImplementedError('embedding regularizers are outside the hot path')
         if self.task not in consts.ALL_TASKS:
             raise ValueError(f'Unknown task type:{self.task}')
+        if len(set(self.emb_dims)) > 1:
+            for net in cfg.nets:
+                if isinstance(net, str) and net in deepnets.EQUAL_WIDTH_NETS:
+                    raise ValueError(f'{net} concatenates the field embeddings on axis 1 and needs one embedding width '
+                                     f'for every categorical column; got widths {self.emb_dims}')
         self._scope = _Scope(self.device, self._seed)
         if self.n_fields:
             self.table = E.EmbeddingTable([c.vocabulary_size for c in self.categorical_columns], self.emb_dim,
-                                          self.device, cfg.embeddings_initializer, self._scope.generator)
+                                          self.device, cfg.embeddings_initializer, self._scope.generator,
+                                          field_dims=self.emb_dims)
             self.table.slot_inits = slot_inits
         self.model_desc = ModelDesc()
         if self.n_fields:
             self.model_desc.add_input('all_categorical_vars', self.n_fields)
             self.model_desc.set_embeddings([c.vocabulary_size for c in self.categorical_columns],
-                                           [self.emb_dim] * self.n_fields, cfg.embedding_dropout)
+                                           list(self.emb_dims), cfg.embedding_dropout)
+            if self.table.ragged:
+                self.model_desc.set_embedding_storage(self.table.dim, self.table.padding_share())
         for c in self.continuous_columns:
             self.model_desc.add_input(c.name, c.input_dim)
         self.model_desc.set_dense(cfg.dense_dropout, False)
@@ -336,7 +340,15 @@ class DeepModel:
         with L.scope_guard(scope):
             embeddings = []
             block = None
-            if self.n_fields:
+            if self.n_fields and self.table.ragged:
+                # fields of different widths: one flat (B, sum D_i) gather feeds flatten_embeddings, the list items
+                # (B, 1, D_i) and, with dropout, concat_embedding_dense, so they all share one mask
+                block = E.RaggedFieldBlock(cat, self.table)
+                if cfg.embedding_dropout > 0 and training:
+                    dropped = E.DropoutFn.apply(block.materialize(), cfg.embedding_dropout, scope.next_seed())
+                    block = E.RaggedFieldBlock(cat, self.table, flat=dropped)
+                embeddings = E.RaggedEmbeddingList(block)
+            elif self.n_fields:
                 block = E.FieldBlock(cat, self.table)
                 if cfg.embedding_dropout > 0 and training:
                     # SpatialDropout1D per field (reference layers.py:878-901): the mask must be shared by
@@ -359,7 +371,12 @@ class DeepModel:
             if 'cin_nets' in cfg.nets and self.n_fields:
                 results['cin_nets'] = deepnets.get('cin_nets')(embeddings, flatten_emb_layer, dense_layer, None, cfg, desc)
             # concat_embedding_dense + bn_concat_emb_dense (reference deepmodel.py:348-361)
-            if block is not None:
+            if isinstance(block, E.RaggedFieldBlock):
+                if block._mat is None:
+                    x = E.RaggedConcatEmbDenseFn.apply(block.table.anchor, dense_layer, block)
+                else:
+                    x = block._mat if dense_layer is None else torch.cat([block._mat, dense_layer], dim=1)
+            elif block is not None:
                 x = E.ConcatEmbDenseFn.apply(block.table.anchor, dense_layer, block)
             elif dense_layer is not None:
                 x = dense_layer
@@ -1220,6 +1237,10 @@ class ModelDesc:
 
     def set_embeddings(self, input_dims, output_dims, embedding_dropout):
         self.embeddings = f'input_dims: {input_dims}\noutput_dims: {output_dims}\ndropout: {embedding_dropout}'
+
+    def set_embedding_storage(self, row_width, padding_share):
+        """Columns of different widths share one table of the widest row; the rest of each row is padding."""
+        self.embeddings += f'\nstored_width: {row_width}\npadding: {100.0 * padding_share:.1f}%'
 
     def set_dense(self, dense_dropout, use_batchnormalization):
         self.dense = f'dropout: {dense_dropout}\nbatch_normalization: {use_batchnormalization}'

@@ -27,6 +27,12 @@ FiBiNet = ['fibi_dnn_nets']
 PNN = ['pnn_nets']
 AFM = ['afm_nets']
 
+# nets that concatenate the field embeddings on axis 1 (or sum each one, linear): with columns of different embedding
+# widths (fixed_embedding_dim=False) Keras's Concatenate refuses their input, so DeepModel refuses them at build time
+EQUAL_WIDTH_NETS = frozenset(['linear', 'cin_nets', 'fm_nets', 'afm_nets', 'opnn_nets', 'ipnn_nets', 'pnn_nets',
+                              'autoint_nets', 'fg_nets', 'fgcnn_cin_nets', 'fgcnn_fm_nets', 'fgcnn_afm_nets',
+                              'fgcnn_ipnn_nets', 'fgcnn_dnn_nets', 'fibi_nets', 'fibi_dnn_nets'])
+
 
 def _concat_embeddings(embeddings, concat_layer_name):
     if embeddings is None or len(embeddings) == 0:

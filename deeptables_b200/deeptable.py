@@ -140,7 +140,9 @@ class DefaultPreprocessor:
             if cfg.auto_scale:
                 lo, hi = float(col.min()), float(col.max())
                 self._scale[c] = (lo, (hi - lo) or 1.0)
-        dim = cfg.embeddings_output_dim if cfg.fixed_embedding_dim else 0
+        # a fixed width of 0 means the default width 4, not CategoricalColumn's fourth root (preprocessor.py:477-478)
+        dim = (cfg.embeddings_output_dim if cfg.embeddings_output_dim > 0 else consts.EMBEDDING_OUT_DIM_DEFAULT) \
+            if cfg.fixed_embedding_dim else 0
         self.categorical_columns = []
         for c in cats:
             vocab = len(self._cat_maps[c]) + 2            # + unseen + reserved (preprocessor.py:333)

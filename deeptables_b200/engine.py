@@ -24,12 +24,24 @@ def _f32(t):
 
 
 class EmbeddingTable:
-    """All categorical columns' embedding matrices in one HBM buffer (uniform embedding dim)."""
+    """All categorical columns' embedding matrices in one HBM buffer of row width ``dim``.
 
-    def __init__(self, vocab_sizes, dim, device, initializer='uniform', generator=None, lazy_adam=True):
+    ``field_dims`` (default: ``dim`` for every field) gives each field's own width D_i <= dim
+    (``fixed_embedding_dim=False``).  Field i then uses columns [0, D_i) of its rows; columns [D_i, dim) are
+    padding that is zero in the weights and the gradient and at its initial value in every optimiser slot.  No
+    kernel writes them, and a zero gradient on zero state is a zero update under every optimiser, so the dense
+    sweeps, the row-wise optimiser kernels and the data-parallel row exchange run unchanged on ``dim``-wide rows."""
+
+    def __init__(self, vocab_sizes, dim, device, initializer='uniform', generator=None, lazy_adam=True,
+                 field_dims=None):
         self.vocab_sizes = [int(v) for v in vocab_sizes]
         self.n_fields = len(self.vocab_sizes)
         self.dim = int(dim)
+        self.field_dims = [self.dim] * self.n_fields if field_dims is None else [int(d) for d in field_dims]
+        if len(self.field_dims) != self.n_fields or not all(1 <= d <= self.dim for d in self.field_dims):
+            raise ValueError(f'field widths {self.field_dims} must be {self.n_fields} values in [1, {self.dim}]')
+        self.ragged = any(d != self.dim for d in self.field_dims)
+        self.dims_host = N.int_array(self.field_dims)
         self.device = torch.device(device)
         offs = [0]
         for v in self.vocab_sizes:
@@ -44,6 +56,9 @@ class EmbeddingTable:
             self.weight.zero_()
         else:
             raise NotImplementedError(f'embeddings_initializer={initializer!r}')
+        for i, d in enumerate(self.field_dims):
+            if d < self.dim:
+                self.weight[offs[i]:offs[i + 1], d:] = 0.0
         self.grad = None
         self.m = None
         self.v = None
@@ -70,9 +85,14 @@ class EmbeddingTable:
             self.last_step = torch.zeros(self.total_rows, dtype=torch.int32, device=self.device)
 
     def field_weight(self, i):
-        """View of the reference's ``embeddings_{i}`` variable."""
+        """View of the reference's ``embeddings_{i}`` variable: (V_i, D_i)."""
         lo, hi = self.row_offsets_host[i], self.row_offsets_host[i + 1]
-        return self.weight[lo:hi]
+        return self.weight[lo:hi, :self.field_dims[i]] if self.ragged else self.weight[lo:hi]
+
+    def padding_share(self):
+        """Fraction of the stored floats that are padding."""
+        pad = sum(v * (self.dim - d) for v, d in zip(self.vocab_sizes, self.field_dims))
+        return pad / max(1, self.total_rows * self.dim)
 
     def check_status(self):
         """TF-CPU raises on an out-of-range id (layers.py:898); the kernels flag it instead."""
@@ -151,6 +171,46 @@ class EmbeddingList:
         if isinstance(i, slice):
             return [mat[:, j:j + 1, :] for j in range(*i.indices(len(self)))]
         return mat[:, i:i + 1, :]
+
+    def __iter__(self):
+        for i in range(len(self)):
+            yield self[i]
+
+
+class RaggedFieldBlock:
+    """Embeddings of fields of different widths (ids + table, ``table.ragged``): what ``flatten_embeddings`` of the
+    reference's embedding list holds, (B, sum D_i).  ``flat`` set: an already materialised (dropped-out) tensor."""
+
+    def __init__(self, idx, table, flat=None):
+        self.idx, self.table, self._mat = idx, table, flat
+
+    def materialize(self):
+        if self._mat is None:
+            self._mat = RaggedConcatEmbDenseFn.apply(self.table.anchor, None, self)
+        return self._mat
+
+
+class RaggedEmbeddingList:
+    """The reference's embedding list for fields of different widths: item i is (B, 1, D_i), a slice of the flat
+    (B, sum D_i) block, so every consumer sees the same gather (and the same dropout mask)."""
+
+    def __init__(self, block):
+        self.block = block
+        cols = [0]
+        for d in block.table.field_dims:
+            cols.append(cols[-1] + d)
+        self._cols = cols
+
+    def __len__(self):
+        return self.block.table.n_fields
+
+    def __getitem__(self, i):
+        if isinstance(i, slice):
+            return [self[j] for j in range(*i.indices(len(self)))]
+        if i < 0:
+            i += len(self)
+        flat = self.block.materialize()
+        return flat[:, self._cols[i]:self._cols[i + 1]].unsqueeze(1)
 
     def __iter__(self):
         for i in range(len(self)):
@@ -301,6 +361,34 @@ class ConcatEmbDenseFn(torch.autograd.Function):
               'concat_emb_dense_bwd')
         _table_grad_done(t)
         return _TableBackwardMixin.finish_tensor_table(t), None, None
+
+
+class RaggedConcatEmbDenseFn(torch.autograd.Function):
+    """flatten_embeddings + concat_embedding_dense over fields of different widths: (B, sum D_i + C)."""
+
+    @staticmethod
+    def forward(ctx, anchor, dense, block):
+        t, idx = block.table, block.idx
+        b, sd = idx.shape[0], sum(t.field_dims)
+        c = 0 if dense is None else dense.shape[1]
+        x = torch.empty(b, sd + c, dtype=torch.float32, device=t.weight.device)
+        check(N.lib.dtb_ragged_concat_emb_dense_fwd(ptr(idx), ptr(t.weight), ptr(t.row_offsets), t.dims_host, ptr(dense),
+                                                    ptr(x), b, t.n_fields, t.dim, c, ptr(t.status), stream_ptr()),
+              'ragged_concat_emb_dense_fwd')
+        ctx.table, ctx.idx, ctx.c = t, idx, c
+        _note_consumer(ctx, t)
+        return x
+
+    @staticmethod
+    def backward(ctx, g):
+        t, idx = ctx.table, ctx.idx
+        gt = _grad_target(t)
+        g = _f32(g)
+        check(N.lib.dtb_ragged_concat_emb_dense_bwd(ptr(idx), ptr(t.row_offsets), t.dims_host, ptr(g), ptr(gt),
+                                                    idx.shape[0], t.n_fields, t.dim, ctx.c, stream_ptr()),
+              'ragged_concat_emb_dense_bwd')
+        _table_grad_done(t)
+        return None, None, None
 
 
 class BatchNormFn(torch.autograd.Function):

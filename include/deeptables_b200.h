@@ -81,6 +81,16 @@ int dtb_concat_emb_dense_fwd(const int32_t* idx, const float* table, const int64
 /* grad_table += dX[:, :F*D] scattered by idx (the dense columns are inputs: no gradient). */
 int dtb_concat_emb_dense_bwd(const int32_t* idx, const int64_t* row_offsets, const float* dX,
                              float* grad_table, int B, int F, int D, int C, void* stream);
+/* The same pair for columns of different widths (fixed_embedding_dim=False, layers.py:862-877).  `table` is
+ * [sum_f V_f, Dmax]; field f uses columns [0, dims_host[f]) of its rows and never touches the rest (padding).
+ * X[b, :] = [e[b,0,0:D_0], ..., e[b,F-1,0:D_{F-1}], dense[b,:]], width W = sum_f D_f + C; C = 0 with dense NULL is
+ * the plain flatten gather.  dims_host: F widths in [1, Dmax], host memory read at call time.  1 <= F <= 960.
+ * The backward scatter-adds dX[:, :sum D_f] into grad_table ([sum_f V_f, Dmax]). */
+int dtb_ragged_concat_emb_dense_fwd(const int32_t* idx, const float* table, const int64_t* row_offsets,
+                                    const int* dims_host, const float* dense, float* X, int B, int F, int Dmax, int C,
+                                    int* status, void* stream);
+int dtb_ragged_concat_emb_dense_bwd(const int32_t* idx, const int64_t* row_offsets, const int* dims_host,
+                                    const float* dX, float* grad_table, int B, int F, int Dmax, int C, void* stream);
 
 /* ---- BatchNormalization(axis=-1) (deepmodel.py:359; layers.py:152; deepnets.py:422) ------ */
 /* Training forward over X[rows, cols]: batch mean / biased variance (two-pass, fp64 accumulate),
