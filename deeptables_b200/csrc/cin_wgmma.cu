@@ -14,7 +14,7 @@
 // data and weight gradients as two fused wgmma kernels in bf16x3 for every precision code.  The data-gradient kernel
 // (one warpgroup per CTA, like the forward) hands dC_k to the weight-gradient kernel already split into the bf16 hi/lo
 // image wgmma reads; the weight-gradient CTA is two warpgroups that share each bulk-copied 64-row block among four
-// m64 A tiles (one or two x0 fields each).
+// m64 A tiles (one or two x0 fields each), fed by a multi-stage ring.
 #include "dtb_common.cuh"
 #include "cin_impl.h"
 #include "wgmma.cuh"
@@ -295,7 +295,11 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
 //     dW_k[i*H + j, l] += sum_m x0[m, i] h_k[m, j] dC_k[m, l]       wgmma: A = x0 h from registers (rows j),
 //                                                                   B = dC_k block as a K-major image (K = m)
 //     Two warpgroups x two m64 A tiles per CTA: one bulk copy of each 64-row block (dC_k image, x0 rows, h_k rows)
-//     into a two-stage ring serves four tiles.  A tile holds one field (H > 32) or two (rows 0-31 and 32-63).
+//     serves four tiles.  A tile holds one field (H > 32) or two (rows 0-31 and 32-63).  The blocks pass through a
+//     ring of up to four stages (as many as fit in shared memory) with a full and an empty mbarrier each: a warpgroup
+//     releases a stage once its MMAs on it are done, and warp 0 refills it.  No CTA-wide barrier sits in the loop, so
+//     the warpgroups drift apart and one builds its A fragments (branch-free, each h value read once per block) while
+//     the other's MMAs run.
 // ==========================================================================================
 
 // dC_k of one 64-row block: K-major image (K = m, N = l < NP) of bf16 hi then lo, core (m/8, l/8) at
@@ -554,28 +558,38 @@ struct CinWgWgradParams {
   int fields_per_tile;   // 2: rows 0-31 of an A tile are field 2t, rows 32-63 field 2t + 1 (H <= 32); else 1
   int hpitch;            // floats between h rows in shared memory
   int hrow_bytes;        // > 0: h rows are copied one by one (that many bytes, to the padded pitch); 0: as one block
+  int stages;            // depth of the ring of row blocks in shared memory (2 .. kWgradMaxStages)
 };
 
 constexpr int kWgradTiles = 4;          // A tiles per CTA: two warpgroups x two m64 accumulators
+constexpr int kWgradMaxStages = 4;
 
 struct CinWgWgradSmem {
   int x0_off, h_off, stage, bar_off, total;
 };
-__host__ __device__ inline CinWgWgradSmem cin_wg_wgrad_layout(int NP, int F, int hpitch) {
+__host__ __device__ inline CinWgWgradSmem cin_wg_wgrad_layout(int NP, int F, int hpitch, int stages) {
   CinWgWgradSmem l;
   l.x0_off = (int)cin_wg_dc_block_bytes(NP);
   l.h_off = l.x0_off + (kWgRows * F * 4 + 127) / 128 * 128;
   l.stage = l.h_off + (kWgRows * hpitch * 4 + 127) / 128 * 128;
-  l.bar_off = 2 * l.stage;
-  l.total = l.bar_off + 16;
+  l.bar_off = stages * l.stage;
+  l.total = l.bar_off + 2 * stages * 8;       // a full and an empty mbarrier per stage
   return l;
+}
+// as many stages as fit in shared memory, 2 to kWgradMaxStages
+static int cin_wg_wgrad_stages(int NP, int F, int hpitch) {
+  int s = kWgradMaxStages;
+  while (s > 2 && cin_wg_wgrad_layout(NP, F, hpitch, s).total > 227 * 1024) --s;
+  return s;
 }
 
 template <int NP>
 __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_constant__ CinWgWgradParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
-  const CinWgWgradSmem lay = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0);
+  const int S = p.stages;
+  const CinWgWgradSmem lay = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0, S);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
+  uint64_t* empty = full + S;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
   const int c2 = 2 * (lane & 3);
   constexpr uint32_t lbo_b = (NP >> 3) * 128;
@@ -584,6 +598,8 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
   // this warp's 16 A rows belong to one field of each of its warpgroup's two tiles; the thread's rows are jw, jw + 8
   const int upper = p.fields_per_tile == 2 && wq >= 2;
   const int jw = (wq - 2 * upper) * 16 + (lane >> 2);
+  // h columns actually read: clamped into the copied rows, so that every shared-memory read stays inside its stage
+  const int jc[2] = {min(jw, H - 1), min(jw + 8, H - 1)};
   int field[2];
   bool tile_on[2], row_ok[2][2];
 #pragma unroll
@@ -595,27 +611,34 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
     row_ok[s][1] = field[s] < F && jw + 8 < H;
     if (field[s] >= F) field[s] = 0;                                 // keeps the x0 reads in range
   }
+  // the first warpgroup always has a tile; the second may have none (last field group), and then leaves at once
+  const bool wg1_on = (blockIdx.x * kWgradTiles + 2) * p.fields_per_tile < F;
   const int64_t n_blocks = (p.BD + kWgRows - 1) / kWgRows;
   const int64_t blk0 = (int64_t)blockIdx.y * p.blocks_per_split;
   int64_t blk1 = blk0 + p.blocks_per_split;
   if (blk1 > n_blocks) blk1 = n_blocks;
+  const int nb = blk1 > blk0 ? (int)(blk1 - blk0) : 0;
 
   if (tid == 0) {
-    tc::mbar_init(&full[0], 1);
-    tc::mbar_init(&full[1], 1);
+    for (int i = 0; i < S; ++i) {
+      tc::mbar_init(&full[i], 1);
+      tc::mbar_init(&empty[i], wg1_on ? 2 : 1);      // one release per working warpgroup
+    }
     tc::fence_barrier_init();
   }
   __syncthreads();
-  // warp 0 brings block blk into stage st: its dC image, its x0 rows and (k >= 1) its h rows
-  auto issue = [&](int64_t blk, int st) {
-    const int64_t gm0 = blk * kWgRows;
+  if (wg == 1 && !wg1_on) return;
+  // warp 0 brings the CTA's block b into stage b % S: its dC image, its x0 rows and (k >= 1) its h rows
+  auto issue = [&](int b) {
+    const int st = b % S;
+    const int64_t gm0 = (blk0 + b) * kWgRows;
     const int rows = p.BD - gm0 < kWgRows ? (int)(p.BD - gm0) : kWgRows;      // a multiple of 4: D divides 64
     uint8_t* sb = smem + st * lay.stage;
     if (lane == 0) {
       uint32_t bytes = cin_wg_dc_block_bytes(NP) + rows * F * 4;
       if (p.h) bytes += rows * (p.hrow_bytes ? p.hrow_bytes : p.ldh * 4);
       tc::mbar_arrive_expect_tx(&full[st], bytes);
-      tc::bulk_g2s(sb, p.dc + blk * cin_wg_dc_block_bytes(NP), cin_wg_dc_block_bytes(NP), &full[st]);
+      tc::bulk_g2s(sb, p.dc + (blk0 + b) * cin_wg_dc_block_bytes(NP), cin_wg_dc_block_bytes(NP), &full[st]);
       tc::bulk_g2s(sb + lay.x0_off, p.x0t + gm0 * F, rows * F * 4, &full[st]);
       if (p.h && !p.hrow_bytes) tc::bulk_g2s(sb + lay.h_off, p.h + gm0 * p.ldh, rows * p.ldh * 4, &full[st]);
     }
@@ -625,40 +648,65 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
         tc::bulk_g2s(sb + lay.h_off + r * p.hpitch * 4, p.h + (gm0 + r) * p.ldh, p.hrow_bytes, &full[st]);
     }
   };
-  if (warp == 0 && blk0 < blk1) issue(blk0, 0);
+  if (warp == 0)
+    for (int b = 0; b < S - 1 && b < nb; ++b) issue(b);
 
   float acc[2][NP / 2];
 #pragma unroll
   for (int s = 0; s < 2; ++s)
 #pragma unroll
     for (int q = 0; q < NP / 2; ++q) acc[s][q] = 0.f;
-  uint32_t n = 0;
-  for (int64_t blk = blk0; blk < blk1; ++blk, ++n) {
-    const int st = n & 1;
-    // the other stage was released by the __syncthreads that ended the previous block
-    if (warp == 0 && blk + 1 < blk1) issue(blk + 1, st ^ 1);
-    const int rows = p.BD - blk * kWgRows < kWgRows ? (int)(p.BD - blk * kWgRows) : kWgRows;
+  // one A fragment set: a warpgroup builds a tile while the other warpgroup's MMAs run
+  uint32_t ahi[kWgRows / 16][4], alo[kWgRows / 16][4];
+  for (int n = 0; n < nb; ++n) {
+    const int st = n % S;
+    const int rows = p.BD - (blk0 + n) * kWgRows < kWgRows ? (int)(p.BD - (blk0 + n) * kWgRows) : kWgRows;
     const uint8_t* sb = smem + st * lay.stage;
     const float* xs = reinterpret_cast<const float*>(sb + lay.x0_off);          // [m][i]
     const float* hs = p.h ? reinterpret_cast<const float*>(sb + lay.h_off) : xs; // [m][j], pitch hp
-    const int hp = p.h ? p.hpitch : F;
+    int hp = p.h ? p.hpitch : F, xp = F;
+    // opaque per block: the row offsets below are recomputed each block instead of held in registers across the loop
+    asm volatile("" : "+r"(hp), "+r"(xp));
     const uint32_t b_hi = tc::smem_u32(sb), b_lo = b_hi + img;
-    tc::mbar_wait(&full[st], (n >> 1) & 1);
+    tc::mbar_wait(&full[st], (n / S) & 1);
+    // the thread's A elements are rows j = jw + 8r and columns m = 16 ks + 8 hb + c2 + e.  Each h[m, j] is read once
+    // per block, each x0[m, field] once per tile; rows past the batch end and rows j >= H are zeroed by a select on
+    // the product (the shared memory behind them may hold anything), so the reads are unconditional and in range.
+    float hv[kWgRows / 16][2][2][2];
+#pragma unroll
+    for (int ks = 0; ks < kWgRows / 16; ++ks)
+#pragma unroll
+      for (int hb = 0; hb < 2; ++hb)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+          for (int r = 0; r < 2; ++r) hv[ks][hb][e][r] = hs[(ks * 16 + hb * 8 + c2 + e) * hp + jc[r]];
 #pragma unroll
     for (int s = 0; s < 2; ++s) {
-      if (!tile_on[s]) continue;
-      uint32_t ahi[kWgRows / 16][4], alo[kWgRows / 16][4];
+      // the MMAs that read the A registers are done; after tile 0 this includes all of the previous block's
+      tc::wgmma_wait<0>();
+      if (s == 0 && n > 0 && wq == 0 && lane == 0) tc::mbar_arrive(&empty[(n - 1) % S]);
+      float xv[kWgRows / 16][2][2];
+#pragma unroll
+      for (int ks = 0; ks < kWgRows / 16; ++ks)
+#pragma unroll
+        for (int hb = 0; hb < 2; ++hb)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) xv[ks][hb][e] = xs[(ks * 16 + hb * 8 + c2 + e) * xp + field[s]];
 #pragma unroll
       for (int ks = 0; ks < kWgRows / 16; ++ks) {
 #pragma unroll
-        for (int f = 0; f < 4; ++f) {
-          const int r = f & 1, j = jw + 8 * r, m = ks * 16 + ((f >> 1) << 3) + c2;
-          const bool ok = row_ok[s][r];
-          const float z0 = ok && m < rows ? xs[m * F + field[s]] * hs[m * hp + j] : 0.f;
-          const float z1 = ok && m + 1 < rows ? xs[(m + 1) * F + field[s]] * hs[(m + 1) * hp + j] : 0.f;
-          tc::split_bf16x2(z0, z1, ahi[ks][f], alo[ks][f]);
+        for (int hb = 0; hb < 2; ++hb) {
+          const int m = ks * 16 + hb * 8 + c2;
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const float z0 = row_ok[s][r] && m < rows ? xv[ks][hb][0] * hv[ks][hb][0][r] : 0.f;
+            const float z1 = row_ok[s][r] && m + 1 < rows ? xv[ks][hb][1] * hv[ks][hb][1][r] : 0.f;
+            tc::split_bf16x2(z0, z1, ahi[ks][2 * hb + r], alo[ks][2 * hb + r]);
+          }
         }
       }
+      // an absent tile (past the last field) runs too, on zero rows, so that no wgmma sits in a branch
       tc::wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < kWgRows / 16; ++ks) {
@@ -669,11 +717,18 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
       }
       tc::wgmma_commit();
     }
-    tc::wgmma_wait<0>();
-    tc::wgmma_fence_acc(acc[0]);
-    tc::wgmma_fence_acc(acc[1]);
-    __syncthreads();
+    // refill the stage of block n - 1 with block n + S - 1 once every working warpgroup has released it
+    if (warp == 0) {
+      const int b = n + S - 1;
+      if (b < nb) {
+        if (b >= S) tc::mbar_wait(&empty[b % S], (b / S - 1) & 1);
+        issue(b);
+      }
+    }
   }
+  tc::wgmma_wait<0>();
+  tc::wgmma_fence_acc(acc[0]);
+  tc::wgmma_fence_acc(acc[1]);
 #pragma unroll
   for (int s = 0; s < 2; ++s) {
     if (!tile_on[s]) continue;
@@ -813,7 +868,7 @@ static int cin_wg_dgrad_launch(const CinWgBwdParams& p, cudaStream_t st) {
 
 template <int NP>
 static int cin_wg_wgrad_launch(const CinWgWgradParams& p, int n_groups, int n_splits, cudaStream_t st) {
-  const int smem = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0).total;
+  const int smem = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0, p.stages).total;
   DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_wgrad_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   cin_wg_wgrad_kernel<NP><<<dim3(n_groups, n_splits), 256, smem, st>>>(p);
   DTB_LAUNCH_OK();
@@ -883,6 +938,7 @@ int cin_wg_bwd(const CinShape& s, const int32_t* idx, const int64_t* row_offsets
         w.hrow_bytes = 0;
         w.hpitch = w.ldh;
       }
+      w.stages = cin_wg_wgrad_stages(np, s.F, w.h ? w.hpitch : 0);
       const int a_tiles = (s.F + w.fields_per_tile - 1) / w.fields_per_tile;
       const int groups = (a_tiles + kWgradTiles - 1) / kWgradTiles;
       int64_t splits = (int64_t)sm_count() / groups;
