@@ -12,9 +12,10 @@
 // operands scaled by exact powers of two (per GEMM row for Z, per layer for W_k), undone on the fp32 accumulator.
 // The saved activations have the layout of the any-shape formulation (x0t, then T_k).  The backward (below) runs the
 // data and weight gradients as two fused wgmma kernels in bf16x3 for every precision code.  The data-gradient kernel
-// (one warpgroup per CTA, like the forward) hands dC_k to the weight-gradient kernel already split into the bf16 hi/lo
-// image wgmma reads; the weight-gradient CTA is two warpgroups that share each bulk-copied 64-row block among four
-// m64 A tiles (one or two x0 fields each), fed by a multi-stage ring.
+// (one warpgroup per CTA, like the forward; one W_k^T chunk serves two x0 fields where 2 H_k <= NPJ) hands dC_k to the
+// weight-gradient kernel already split into the bf16 hi/lo image wgmma reads; the weight-gradient CTA is two
+// warpgroups that share each bulk-copied 64-row block among four m64 A tiles (one or two x0 fields each), fed by a
+// multi-stage ring.
 #include "dtb_common.cuh"
 #include "cin_impl.h"
 #include "wgmma.cuh"
@@ -289,6 +290,8 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
 //     dC_k = (d_pooled part + dh_{k+1}) * act'(T_k)                 registers, accumulator fragment layout
 //     dZ_{k,i}[m, j] = sum_l dC_k[m, l] W_k[i*H + j, l]             wgmma: A = dC_k from registers, B = W_k^T chunk
 //     dx0[m, i] += sum_j dZ h_k[m, j] ;  dh_k[m, j] += dZ x0[m, i]   registers (dh_k feeds dC_{k-1})
+//     N = NPJ, the padded largest H.  Where 2 H_k <= NPJ, one chunk holds fields 2t and 2t + 1 (columns [0, NPJ/2) and
+//     [NPJ/2, NPJ)), so a narrow layer (layer 0 at the headline shape) runs half the MMAs and copies half the weights.
 //     dC_k is stored as the bf16 hi/lo image the weight gradient multiplies (below), its column sums go to d_bias,
 //     and dx0 is scattered into grad_table.
 //   wgrad, per (layer k, group of x0 fields, row split):
@@ -309,7 +312,7 @@ __host__ __device__ inline uint32_t cin_wg_dc_block_bytes(int NP) { return (uint
 struct CinWgBwdParams {
   const int32_t* idx;
   const int64_t* row_offsets;
-  const uint8_t* wpack;      // per layer, per field: W_k^T image [NPJ x LP], hi then lo
+  const uint8_t* wpack;      // per layer, per chunk of fpc x0 fields: W_k^T image [NPJ x LP], hi then lo
   const float* d_pooled;
   const float* saved;        // x0t [B*D, F] then T_k [B*D, L_k]
   float* grad_table;
@@ -317,22 +320,27 @@ struct CinWgBwdParams {
   float* dbias;              // null, or d_bias of all layers (offsets bias_off)
   int B, D, F, n_layers, act, P, NPdc;
   int L[kCinMaxLayers], LP[kCinMaxLayers], H[kCinMaxLayers], hid_n[kCinMaxLayers];
+  int fpc[kCinMaxLayers];    // x0 fields per weight chunk: 2 when 2 H_k <= NPJ, else 1
+  int nch[kCinMaxLayers];    // weight chunks of layer k: ceil(F / fpc)
   int pool_lo[kCinMaxLayers], pool_n[kCinMaxLayers], pcol0[kCinMaxLayers];
   unsigned long long wpack_off[kCinMaxLayers], saved_off[kCinMaxLayers], dc_off[kCinMaxLayers], bias_off[kCinMaxLayers];
 };
 
-// W_k [F*H, L] -> per field i: K-major image of B[n][kk] = W_k[i*H + n, kk] (n < H, kk < L, else 0), N = NPJ, K = LP
+// W_k [F*H, L] -> per chunk c of fpc x0 fields: K-major image of B[n][kk] = W_k[i*H + j, kk], N = NPJ, K = LP, where
+// field i = c*fpc + n / (NPJ/fpc) and j = n % (NPJ/fpc); zero for j >= H, i >= F or kk >= L
 __global__ void cin_wg_pack_t_kernel(const float* __restrict__ w, uint8_t* __restrict__ out, int F, int H, int L, int LP,
-                                     int NPJ) {
+                                     int NPJ, int fpc) {
   const int64_t per_chunk = (int64_t)NPJ * LP;
-  const int64_t total = per_chunk * F;
+  const int64_t total = per_chunk * ((F + fpc - 1) / fpc);
+  const int half = NPJ / fpc;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const int i = (int)(t / per_chunk);
-    const int rem = (int)(t - (int64_t)i * per_chunk);
+    const int c = (int)(t / per_chunk);
+    const int rem = (int)(t - (int64_t)c * per_chunk);
     const int n = rem / LP, kk = rem - n * LP;          // kk fastest: coalesced reads of W rows
-    const float v = (n < H && kk < L) ? w[((int64_t)i * H + n) * L + kk] : 0.f;
+    const int sub = n / half, j = n - sub * half, i = c * fpc + sub;
+    const float v = (i < F && j < H && kk < L) ? w[((int64_t)i * H + j) * L + kk] : 0.f;
     const int64_t off = ((int64_t)(kk >> 3) * (NPJ >> 3) + (n >> 3)) * 128 + (n & 7) * 16 + (kk & 7) * 2;
-    uint8_t* base = out + (int64_t)i * per_chunk * 4;
+    uint8_t* base = out + (int64_t)c * per_chunk * 4;
     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
     *reinterpret_cast<__nv_bfloat16*>(base + off) = hi;
     *reinterpret_cast<__nv_bfloat16*>(base + per_chunk * 2 + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
@@ -398,6 +406,14 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
       dxs[e] = 0.f;
     }
     __syncthreads();
+    // the thread's two accumulator rows r0, r0 + 8: inside the batch?  which batch row?
+    bool row_ok[2];
+    int64_t row_b[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      row_ok[h] = gm0 + r0 + 8 * h < BD;
+      row_b[h] = row_ok[h] ? (gm0 + r0 + 8 * h) / D : 0;
+    }
     float dh[NPJ / 2];                   // gradient wrt h_{k+1}, accumulator fragment order (columns j)
 #pragma unroll
     for (int q = 0; q < NPJ / 2; ++q) dh[q] = 0.f;
@@ -408,25 +424,34 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
       {
         const float* T = p.saved + p.saved_off[k];
         uint8_t* img = p.dc + p.dc_off[k] + (size_t)tile * cin_wg_dc_block_bytes(NPdc);
+        // All global reads of the layer come first, in a loop with no store and no branch around a load: a load
+        // under a branch whose value a shuffle consumes at once, or one that a dC image store (which may alias T) must
+        // precede, waits out its own memory round trip.  Rows past the batch end and columns l >= L read in-range
+        // addresses and are zeroed by selects.
+        const int pool_lo = p.pool_lo[k], pool_hi = pool_lo + p.pool_n[k], hid = p.hid_n[k];
+        const bool relu = p.act == DTB_ACT_RELU;
+        int64_t tb[2], pb[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          tb[h] = row_ok[h] ? (gm0 + r0 + 8 * h) * L : 0;
+          pb[h] = row_b[h] * p.P + p.pcol0[k] - pool_lo;
+        }
+        float gq[kWgMaxNP / 2];
+#pragma unroll
+        for (int q = 0; q < kWgMaxNP / 2; ++q) {
+          const int h = (q >> 1) & 1, l = 8 * (q >> 2) + c2 + (q & 1);
+          const bool ok = row_ok[h] && l < L, pooled = ok && l >= pool_lo && l < pool_hi;
+          const float tv = __ldg(T + (ok ? tb[h] + l : 0));
+          const float dp = __ldg(p.d_pooled + (pooled ? pb[h] + l : 0));
+          float v = pooled ? 0.f + dp : 0.f;
+          if (q < NPJ / 2) v = ok && l < hid ? v + dh[q] : v;
+          gq[q] = ok && !(relu && !(tv > 0.f)) ? v : 0.f;
+        }
         float bs[2] = {0.f, 0.f};
 #pragma unroll
         for (int q = 0; q < kWgMaxNP / 2; q += 2) {
           const int row = r0 + (((q >> 1) & 1) << 3), l = 8 * (q >> 2) + c2;
-          const int64_t gm = gm0 + row;
-          float g[2] = {0.f, 0.f};
-          if (gm < BD && l < LP) {
-            const int64_t b = gm / D;
-#pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const int lu = l + u;
-              if (lu < L) {
-                if (lu >= p.pool_lo[k] && lu < p.pool_lo[k] + p.pool_n[k])
-                  g[u] += __ldg(p.d_pooled + b * p.P + p.pcol0[k] + lu - p.pool_lo[k]);
-                if (lu < p.hid_n[k] && q + u < NPJ / 2) g[u] += dh[q + u];
-                if (p.act == DTB_ACT_RELU && !(T[gm * L + lu] > 0.f)) g[u] = 0.f;
-              }
-            }
-          }
+          const float g[2] = {gq[q], gq[q + 1]};
           tc::split_bf16x2(g[0], g[1], ahi[q >> 3][(q >> 1) & 3], alo[q >> 3][(q >> 1) & 3]);
           // dC image: the lane of the partner row (lane ^ 4) swaps one value, so each lane holds rows (2t, 2t + 1) of
           // one column and stores their hi and lo pairs as one word each.  Only the stores are conditional: a branch
@@ -474,15 +499,16 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
           dh[q] = 0.f;
         }
       }
-      for (int i = 0; i < F; ++i, ++chunk) {
+      const int fpc = p.fpc[k], nch = p.nch[k];
+      for (int t = 0; t < nch; ++t, ++chunk) {
         if (tid == 0) {
-          int nk = k, ni = i + 1;
+          int nk = k, nt = t + 1;
           bool more = true;
-          if (ni == F) {
-            ni = 0;
+          if (nt == nch) {
+            nt = 0;
             if (--nk < 0) { nk = K0; more = tile + (int)gridDim.x < n_tiles; }
           }
-          if (more) issue(chunk + 1, nk, ni);
+          if (more) issue(chunk + 1, nk, nt);
         }
         float acc[NPJ / 2];
 #pragma unroll
@@ -504,20 +530,62 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
         tc::wgmma_wait<0>();
         tc::wgmma_fence_acc(acc);
         // dx0[m, i] += sum_j dZ h ; dh[m, j] += dZ x0[m, i]
-        const float x_a = x0s[r0 * F + i], x_b = x0s[(r0 + 8) * F + i];
-        float s_a = 0.f, s_b = 0.f;
+        if (fpc == 2) {
+          // field 2t in columns [0, NPJ/2), field 2t + 1 in [NPJ/2, NPJ): acc[q] and acc[q + Q] are the same j of the
+          // two fields, and hh / dh past Q are zero (H <= NPJ/2).  A missing field 2t + 1 (odd F) has zero weights.
+          constexpr int Q = NPJ / 4;
+          const int i0 = 2 * t;
+          const bool two = i0 + 1 < F;
+          const int i1 = two ? i0 + 1 : i0;
+          const float x_a0 = x0s[r0 * F + i0], x_b0 = x0s[(r0 + 8) * F + i0];
+          const float x_a1 = two ? x0s[r0 * F + i1] : 0.f, x_b1 = two ? x0s[(r0 + 8) * F + i1] : 0.f;
+          float s_a0 = 0.f, s_b0 = 0.f, s_a1 = 0.f, s_b1 = 0.f;
 #pragma unroll
-        for (int q = 0; q < NPJ / 2; ++q) {
-          if ((q >> 1) & 1) { s_b += acc[q] * hh[q]; dh[q] += acc[q] * x_b; }
-          else              { s_a += acc[q] * hh[q]; dh[q] += acc[q] * x_a; }
-        }
-        s_a += __shfl_xor_sync(0xffffffffu, s_a, 1);
-        s_a += __shfl_xor_sync(0xffffffffu, s_a, 2);
-        s_b += __shfl_xor_sync(0xffffffffu, s_b, 1);
-        s_b += __shfl_xor_sync(0xffffffffu, s_b, 2);
-        if ((lane & 3) == 0) {
-          dxs[r0 * F + i] += s_a;
-          dxs[(r0 + 8) * F + i] += s_b;
+          for (int q = 0; q < Q; ++q) {
+            if ((q >> 1) & 1) {
+              s_b0 += acc[q] * hh[q];
+              s_b1 += acc[q + Q] * hh[q];
+              dh[q] += acc[q] * x_b0;
+              dh[q] += acc[q + Q] * x_b1;
+            } else {
+              s_a0 += acc[q] * hh[q];
+              s_a1 += acc[q + Q] * hh[q];
+              dh[q] += acc[q] * x_a0;
+              dh[q] += acc[q + Q] * x_a1;
+            }
+          }
+#pragma unroll
+          for (int o = 1; o <= 2; o <<= 1) {
+            s_a0 += __shfl_xor_sync(0xffffffffu, s_a0, o);
+            s_b0 += __shfl_xor_sync(0xffffffffu, s_b0, o);
+            s_a1 += __shfl_xor_sync(0xffffffffu, s_a1, o);
+            s_b1 += __shfl_xor_sync(0xffffffffu, s_b1, o);
+          }
+          if ((lane & 3) == 0) {
+            dxs[r0 * F + i0] += s_a0;
+            dxs[(r0 + 8) * F + i0] += s_b0;
+            if (two) {
+              dxs[r0 * F + i1] += s_a1;
+              dxs[(r0 + 8) * F + i1] += s_b1;
+            }
+          }
+        } else {
+          const int i = t;
+          const float x_a = x0s[r0 * F + i], x_b = x0s[(r0 + 8) * F + i];
+          float s_a = 0.f, s_b = 0.f;
+#pragma unroll
+          for (int q = 0; q < NPJ / 2; ++q) {
+            if ((q >> 1) & 1) { s_b += acc[q] * hh[q]; dh[q] += acc[q] * x_b; }
+            else              { s_a += acc[q] * hh[q]; dh[q] += acc[q] * x_a; }
+          }
+          s_a += __shfl_xor_sync(0xffffffffu, s_a, 1);
+          s_a += __shfl_xor_sync(0xffffffffu, s_a, 2);
+          s_b += __shfl_xor_sync(0xffffffffu, s_b, 1);
+          s_b += __shfl_xor_sync(0xffffffffu, s_b, 2);
+          if ((lane & 3) == 0) {
+            dxs[r0 * F + i] += s_a;
+            dxs[(r0 + 8) * F + i] += s_b;
+          }
         }
         __syncthreads();
       }
@@ -839,9 +907,14 @@ static int cin_wg_npj(const CinShape& s) {
   while (np < hp) np *= 2;
   return np;
 }
+// x0 fields per W_k^T chunk of the data gradient: two when both fit in the NPJ columns
+static int cin_wg_dgrad_fpc(const CinShape& s, int k) { return 2 * s.H[k] <= cin_wg_npj(s) ? 2 : 1; }
 static size_t cin_wg_pack_t_bytes(const CinShape& s) {
   size_t b = 0;
-  for (int k = 0; k < s.n_layers; ++k) b += (size_t)s.F * cin_wg_npj(s) * round_up16(s.L[k]) * 4;
+  for (int k = 0; k < s.n_layers; ++k) {
+    const int fpc = cin_wg_dgrad_fpc(s, k);
+    b += (size_t)((s.F + fpc - 1) / fpc) * cin_wg_npj(s) * round_up16(s.L[k]) * 4;
+  }
   return (b + 255) / 256 * 256;
 }
 // dC_k images of every layer: whole 64-row blocks of cin_wg_np columns (4 bytes per element, hi + lo)
@@ -902,14 +975,16 @@ int cin_wg_bwd(const CinShape& s, const int32_t* idx, const int64_t* row_offsets
     size_t woff = 0;
     for (int k = 0; k < s.n_layers; ++k) {
       p.L[k] = s.L[k]; p.LP[k] = round_up16(s.L[k]); p.H[k] = s.H[k]; p.hid_n[k] = k + 1 < s.n_layers ? s.H[k + 1] : 0;
+      p.fpc[k] = cin_wg_dgrad_fpc(s, k); p.nch[k] = (s.F + p.fpc[k] - 1) / p.fpc[k];
       p.pool_lo[k] = s.pool_lo[k]; p.pool_n[k] = s.pool_n[k]; p.pcol0[k] = s.pcol0[k];
       p.wpack_off[k] = woff; p.saved_off[k] = saved_off[k]; p.dc_off[k] = dc_off[k]; p.bias_off[k] = s.b_off[k];
-      const int64_t total = (int64_t)s.F * npj * p.LP[k];
+      const int64_t total = (int64_t)p.nch[k] * npj * p.LP[k];
       int blocks = (int)((total + 255) / 256);
       if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-      cin_wg_pack_t_kernel<<<blocks, 256, 0, st>>>(weights + s.w_off[k], ws + woff, s.F, s.H[k], s.L[k], p.LP[k], npj);
+      cin_wg_pack_t_kernel<<<blocks, 256, 0, st>>>(weights + s.w_off[k], ws + woff, s.F, s.H[k], s.L[k], p.LP[k], npj,
+                                                   p.fpc[k]);
       DTB_LAUNCH_OK();
-      woff += (size_t)s.F * npj * p.LP[k] * 4;
+      woff += (size_t)p.nch[k] * npj * p.LP[k] * 4;
     }
     int rc;
     switch (npj) {

@@ -6,6 +6,7 @@ dtb_cin_bwd_phase calls with L2 flushed before each backward, as bench.py does.
 
 Prints ms per kernel and TFLOP/s per kernel: executed (what the tensor cores run: padded tiles, bf16x3 = 3 passes) and
 algorithmic (the FMAs of the math alone), both counted from the shape below, plus the card name and power limit.
+For the data gradient it also prints the bytes of weight chunks copied into shared memory and their rate.
 """
 import argparse
 import ctypes
@@ -20,20 +21,35 @@ sys.path.insert(0, ROOT)
 F, D, SIZES = 26, 16, (128, 128, 128)
 
 
-def flop_counts(b):
-    """FMA counts per kernel: {name: (executed, algorithmic)}; mirrors the tiling of csrc/cin_wgmma.cu."""
+def _shape(b):
     from oracle import layers_ref as L
     bd = b * D
     n_blocks = (bd + 63) // 64
     H = L.cin_field_nums(F, SIZES, False)[:len(SIZES)]
-    np_ = 16
-    while np_ < max(SIZES):
-        np_ *= 2
     npj = 16
     while npj < max((h + 15) // 16 * 16 for h in H):
         npj *= 2
+    return bd, n_blocks, H, npj
+
+
+def dgrad_chunks(b):
+    """(weight chunks per layer, their bytes) one 64-row tile of cin_wg_dgrad_kernel multiplies, and the tile count.
+    A chunk is the W_k^T image of one x0 field, or of two where 2 H_k <= NPJ: NPJ x LP, bf16 hi + lo."""
+    bd, n_blocks, H, npj = _shape(b)
+    nch = [(F + 1) // 2 if 2 * h <= npj else F for h in H]
+    nbytes = sum(c * npj * ((s + 15) // 16 * 16) * 4 for c, s in zip(nch, SIZES))
+    return nch, nbytes, n_blocks
+
+
+def flop_counts(b):
+    """FMA counts per kernel: {name: (executed, algorithmic)}; mirrors the tiling of csrc/cin_wgmma.cu."""
+    bd, n_blocks, H, npj = _shape(b)
+    np_ = 16
+    while np_ < max(SIZES):
+        np_ *= 2
     out = {}
-    exe = sum(n_blocks * 64 * F * npj * ((s + 15) // 16 * 16) * 3 for s in SIZES)
+    nch, _, _ = dgrad_chunks(b)
+    exe = sum(n_blocks * 64 * c * npj * ((s + 15) // 16 * 16) * 3 for c, s in zip(nch, SIZES))
     out['cin_wg_dgrad_kernel'] = (exe, sum(bd * F * h * s for h, s in zip(H, SIZES)))
     for k, (h, s) in enumerate(zip(H, SIZES)):
         fpt = 2 if h <= 32 else 1
@@ -130,6 +146,11 @@ def main():
             wg_total += ms
         res['kernels'][key] = {'ms': round(ms, 4), 'executed_tflops': round(2 * exe / ms * 1e-9, 1),
                                'algorithmic_tflops': round(2 * alg / ms * 1e-9, 1)}
+        if key == 'cin_wg_dgrad_kernel':
+            # weight chunks bulk-copied from L2 into shared memory, one copy per tile and chunk
+            _, tile_bytes, n_tiles = dgrad_chunks(b)
+            gb = tile_bytes * n_tiles * 1e-9
+            res['kernels'][key].update(weight_chunk_gb=round(gb, 2), weight_chunk_gbps=round(gb / ms * 1e3, 1))
     res['wgrad_ms_total'] = round(wg_total, 4)
     print(json.dumps(res, indent=1))
 
