@@ -14,13 +14,14 @@
 // data and weight gradients as two fused wgmma kernels in bf16x3 for every precision code.  The data-gradient kernel
 // (one warpgroup per CTA, like the forward; one W_k^T chunk serves two x0 fields where 2 H_k <= NPJ) hands dC_k to the
 // weight-gradient kernel already split into the bf16 hi/lo image wgmma reads; the weight-gradient CTA is two
-// warpgroups that share each bulk-copied 64-row block among four m64 A tiles (one or two x0 fields each), fed by a
-// multi-stage ring.
+// warpgroups that share each copied 64-row block among four m64 A tiles (one or two x0 fields each), fed by a
+// multi-stage ring that a third, producer warpgroup refills.
 #include "dtb_common.cuh"
 #include "cin_impl.h"
 #include "wgmma.cuh"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cudaTypedefs.h>      // CUtensorMap, PFN_cuTensorMapEncodeTiled
 
 namespace dtb {
 
@@ -297,12 +298,16 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
 //   wgrad, per (layer k, group of x0 fields, row split):
 //     dW_k[i*H + j, l] += sum_m x0[m, i] h_k[m, j] dC_k[m, l]       wgmma: A = x0 h from registers (rows j),
 //                                                                   B = dC_k block as a K-major image (K = m)
-//     Two warpgroups x two m64 A tiles per CTA: one bulk copy of each 64-row block (dC_k image, x0 rows, h_k rows)
-//     serves four tiles.  A tile holds one field (H > 32) or two (rows 0-31 and 32-63).  The blocks pass through a
-//     ring of up to four stages (as many as fit in shared memory) with a full and an empty mbarrier each: a warpgroup
-//     releases a stage once its MMAs on it are done, and warp 0 refills it.  No CTA-wide barrier sits in the loop, so
-//     the warpgroups drift apart and one builds its A fragments (branch-free, each h value read once per block) while
-//     the other's MMAs run.
+//     Two consumer warpgroups x two m64 A tiles per CTA, plus a producer warpgroup: one copy of each 64-row block
+//     (dC_k image and x0 rows by bulk copy; for k >= 1 the h_k rows by one 2-D tensor copy of their first hpitch
+//     columns, or whole rows by bulk copy when ldh % 4 != 0) serves four tiles.  A tile holds one field (H > 32) or
+//     two (rows 0-31 and 32-63).  The blocks pass through a ring of up to four stages (as many as fit in shared
+//     memory) with a full and an empty mbarrier each.  One producer thread owns every empty-barrier wait and every
+//     refill (setmaxnreg: 24 registers for it, 240 for the consumers); the consumers only wait on full barriers,
+//     build A fragments (branch-free, each h value read once per block) and issue wgmma, releasing a stage once their
+//     MMAs on it are done.  No CTA-wide barrier sits in the loop, so one warpgroup builds while the other multiplies.
+//     A last field group with tiles for one warpgroup only runs them on both, on alternate blocks, and gets a longer
+//     row split than the full groups, so that all SMs have work and finish together.
 // ==========================================================================================
 
 // dC_k of one 64-row block: K-major image (K = m, N = l < NP) of bf16 hi then lo, core (m/8, l/8) at
@@ -617,20 +622,28 @@ __global__ void __launch_bounds__(128) cin_wg_dgrad_kernel(const __grid_constant
 }
 
 struct CinWgWgradParams {
+  CUtensorMap hmap;      // htensor: T_{k-1} as a [B*D, ldh] fp32 tensor, box hpitch columns x 64 rows
   const float* x0t;      // [B*D, F]
   const float* h;        // T_{k-1} [B*D, ldh] (its first H columns are h_k); null for k = 0, where h_0 = x0
   const uint8_t* dc;     // dC_k images, one per 64-row block
   float* dw;             // dW_k [F*H, L]
   int64_t BD;
-  int F, H, L, ldh, blocks_per_split;
+  int F, H, L, ldh;
   int fields_per_tile;   // 2: rows 0-31 of an A tile are field 2t, rows 32-63 field 2t + 1 (H <= 32); else 1
   int hpitch;            // floats between h rows in shared memory
-  int hrow_bytes;        // > 0: h rows are copied one by one (that many bytes, to the padded pitch); 0: as one block
+  int htensor;           // 1: an h block arrives as one tensor copy of its first hpitch columns; 0: whole rows (ldh)
   int stages;            // depth of the ring of row blocks in shared memory (2 .. kWgradMaxStages)
+  int groups;            // field groups of kWgradTiles A tiles; CTAs [0, (groups-1) splits) run the full ones
+  int splits, blocks_per_split;            // row splits of each of the first groups - 1 field groups
+  int last_splits, last_blocks_per_split;  // and of the last one
+  int last_pair;         // 1: the last group has tiles for one warpgroup only; both run them, on alternate blocks
 };
 
 constexpr int kWgradTiles = 4;          // A tiles per CTA: two warpgroups x two m64 accumulators
 constexpr int kWgradMaxStages = 4;
+constexpr int kWgradThreads = 384;      // consumer warpgroups 0 and 1, producer warpgroup 2
+// the registers the CTA gets at launch (384 x 168) are shared out again: 2 x 128 x 240 + 128 x 24 = 384 x 168
+constexpr int kWgradConsumerRegs = 240, kWgradProducerRegs = 24;
 
 struct CinWgWgradSmem {
   int x0_off, h_off, stage, bar_off, total;
@@ -652,17 +665,73 @@ static int cin_wg_wgrad_stages(int NP, int F, int hpitch) {
 }
 
 template <int NP>
-__global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_constant__ CinWgWgradParams p) {
+__global__ void __launch_bounds__(kWgradThreads, 1) cin_wg_wgrad_kernel(const __grid_constant__ CinWgWgradParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int S = p.stages;
   const CinWgWgradSmem lay = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0, S);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
   uint64_t* empty = full + S;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
+  const int F = p.F, H = p.H;
+  // CTA -> field group g and row split y.  The full groups come first, split-major, so that the CTAs reading the same
+  // rows run side by side; the last group has its own split count.
+  const int nfull = p.groups - 1;
+  int g, y, bps;
+  if ((int)blockIdx.x < nfull * p.splits) {
+    g = (int)blockIdx.x % nfull; y = (int)blockIdx.x / nfull; bps = p.blocks_per_split;
+  } else {
+    g = nfull; y = (int)blockIdx.x - nfull * p.splits; bps = p.last_blocks_per_split;
+  }
+  // pair: both warpgroups run the group's first two tiles, warpgroup w on the blocks n = w mod 2
+  const bool pair = g == nfull && p.last_pair;
+  // otherwise the first warpgroup always has a tile; the second may have none (last field group) and then leaves
+  const bool wg1_on = pair || (g * kWgradTiles + 2) * p.fields_per_tile < F;
+  const int64_t n_blocks = (p.BD + kWgRows - 1) / kWgRows;
+  const int64_t blk0 = (int64_t)y * bps;
+  int64_t blk1 = blk0 + bps;
+  if (blk1 > n_blocks) blk1 = n_blocks;
+  const int nb = blk1 > blk0 ? (int)(blk1 - blk0) : 0;
+
+  if (tid == 0) {
+    for (int i = 0; i < S; ++i) {
+      tc::mbar_init(&full[i], 1);
+      tc::mbar_init(&empty[i], wg1_on && !pair ? 2 : 1);      // one release per warpgroup that reads the block
+    }
+    tc::fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    // producer: one thread brings block b into stage b % S (its dC image, its x0 rows and, k >= 1, its h rows) once
+    // the readers of block b - S have released the stage
+    tc::setmaxnreg_dec<kWgradProducerRegs>();
+    if (tid == 2 * 128) {
+      for (int b = 0; b < nb; ++b) {
+        const int st = b % S;
+        const int64_t gm0 = (blk0 + b) * kWgRows;
+        const int rows = p.BD - gm0 < kWgRows ? (int)(p.BD - gm0) : kWgRows;      // a multiple of 4: D divides 64
+        uint8_t* sb = smem + st * lay.stage;
+        uint32_t bytes = cin_wg_dc_block_bytes(NP) + rows * F * 4;
+        if (p.h) bytes += p.htensor ? kWgRows * p.hpitch * 4 : rows * p.ldh * 4;    // a tensor box always lands whole
+        if (b >= S) tc::mbar_wait(&empty[st], (b / S - 1) & 1);
+        tc::mbar_arrive_expect_tx(&full[st], bytes);
+        tc::bulk_g2s(sb, p.dc + (blk0 + b) * cin_wg_dc_block_bytes(NP), cin_wg_dc_block_bytes(NP), &full[st]);
+        tc::bulk_g2s(sb + lay.x0_off, p.x0t + gm0 * F, rows * F * 4, &full[st]);
+        if (p.h) {
+          if (p.htensor) tc::tma_load_2d(sb + lay.h_off, &p.hmap, 0, (int)gm0, &full[st]);
+          else tc::bulk_g2s(sb + lay.h_off, p.h + gm0 * p.ldh, rows * p.ldh * 4, &full[st]);
+        }
+      }
+    }
+    return;
+  }
+  tc::setmaxnreg_inc<kWgradConsumerRegs>();
+  if (wg == 1 && !wg1_on) return;
+
+  // consumers: wait for full stages, build A, issue wgmma, release stages
   const int c2 = 2 * (lane & 3);
   constexpr uint32_t lbo_b = (NP >> 3) * 128;
   constexpr uint32_t img = NP * kWgRows * 2;
-  const int F = p.F, H = p.H;
   // this warp's 16 A rows belong to one field of each of its warpgroup's two tiles; the thread's rows are jw, jw + 8
   const int upper = p.fields_per_tile == 2 && wq >= 2;
   const int jw = (wq - 2 * upper) * 16 + (lane >> 2);
@@ -672,52 +741,17 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
   bool tile_on[2], row_ok[2][2];
 #pragma unroll
   for (int s = 0; s < 2; ++s) {
-    const int t = blockIdx.x * kWgradTiles + wg * 2 + s;
+    const int t = g * kWgradTiles + (pair ? 0 : wg * 2) + s;
     tile_on[s] = t * p.fields_per_tile < F;                         // warpgroup-uniform
     field[s] = t * p.fields_per_tile + upper;
     row_ok[s][0] = field[s] < F && jw < H;
     row_ok[s][1] = field[s] < F && jw + 8 < H;
     if (field[s] >= F) field[s] = 0;                                 // keeps the x0 reads in range
   }
-  // the first warpgroup always has a tile; the second may have none (last field group), and then leaves at once
-  const bool wg1_on = (blockIdx.x * kWgradTiles + 2) * p.fields_per_tile < F;
-  const int64_t n_blocks = (p.BD + kWgRows - 1) / kWgRows;
-  const int64_t blk0 = (int64_t)blockIdx.y * p.blocks_per_split;
-  int64_t blk1 = blk0 + p.blocks_per_split;
-  if (blk1 > n_blocks) blk1 = n_blocks;
-  const int nb = blk1 > blk0 ? (int)(blk1 - blk0) : 0;
-
-  if (tid == 0) {
-    for (int i = 0; i < S; ++i) {
-      tc::mbar_init(&full[i], 1);
-      tc::mbar_init(&empty[i], wg1_on ? 2 : 1);      // one release per working warpgroup
-    }
-    tc::fence_barrier_init();
-  }
-  __syncthreads();
-  if (wg == 1 && !wg1_on) return;
-  // warp 0 brings the CTA's block b into stage b % S: its dC image, its x0 rows and (k >= 1) its h rows
-  auto issue = [&](int b) {
-    const int st = b % S;
-    const int64_t gm0 = (blk0 + b) * kWgRows;
-    const int rows = p.BD - gm0 < kWgRows ? (int)(p.BD - gm0) : kWgRows;      // a multiple of 4: D divides 64
-    uint8_t* sb = smem + st * lay.stage;
-    if (lane == 0) {
-      uint32_t bytes = cin_wg_dc_block_bytes(NP) + rows * F * 4;
-      if (p.h) bytes += rows * (p.hrow_bytes ? p.hrow_bytes : p.ldh * 4);
-      tc::mbar_arrive_expect_tx(&full[st], bytes);
-      tc::bulk_g2s(sb, p.dc + (blk0 + b) * cin_wg_dc_block_bytes(NP), cin_wg_dc_block_bytes(NP), &full[st]);
-      tc::bulk_g2s(sb + lay.x0_off, p.x0t + gm0 * F, rows * F * 4, &full[st]);
-      if (p.h && !p.hrow_bytes) tc::bulk_g2s(sb + lay.h_off, p.h + gm0 * p.ldh, rows * p.ldh * 4, &full[st]);
-    }
-    if (p.h && p.hrow_bytes) {
-      __syncwarp();
-      for (int r = lane; r < rows; r += 32)
-        tc::bulk_g2s(sb + lay.h_off + r * p.hpitch * 4, p.h + (gm0 + r) * p.ldh, p.hrow_bytes, &full[st]);
-    }
-  };
-  if (warp == 0)
-    for (int b = 0; b < S - 1 && b < nb; ++b) issue(b);
+  const int n0 = pair ? wg : 0, step = pair ? 2 : 1;
+  // rows of the CTA's blocks, counted from its first block.  It fits an int: the dC images alone take 64 B per row
+  // (NP >= 16), so no device holds 2^31 rows.
+  const int rows_end = (int)((blk1 * kWgRows < p.BD ? blk1 * kWgRows : p.BD) - blk0 * kWgRows);
 
   float acc[2][NP / 2];
 #pragma unroll
@@ -726,9 +760,9 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
     for (int q = 0; q < NP / 2; ++q) acc[s][q] = 0.f;
   // one A fragment set: a warpgroup builds a tile while the other warpgroup's MMAs run
   uint32_t ahi[kWgRows / 16][4], alo[kWgRows / 16][4];
-  for (int n = 0; n < nb; ++n) {
+  for (int n = n0; n < nb; n += step) {
     const int st = n % S;
-    const int rows = p.BD - (blk0 + n) * kWgRows < kWgRows ? (int)(p.BD - (blk0 + n) * kWgRows) : kWgRows;
+    const int rows = min(rows_end - n * kWgRows, kWgRows);
     const uint8_t* sb = smem + st * lay.stage;
     const float* xs = reinterpret_cast<const float*>(sb + lay.x0_off);          // [m][i]
     const float* hs = p.h ? reinterpret_cast<const float*>(sb + lay.h_off) : xs; // [m][j], pitch hp
@@ -751,9 +785,10 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
           for (int r = 0; r < 2; ++r) hv[ks][hb][e][r] = hs[(ks * 16 + hb * 8 + c2 + e) * hp + jc[r]];
 #pragma unroll
     for (int s = 0; s < 2; ++s) {
-      // the MMAs that read the A registers are done; after tile 0 this includes all of the previous block's
+      // the MMAs that read the A registers are done; before tile 0 this includes all of the warpgroup's previous
+      // block's, whose stage is released (the producer may refill it with block n - step + S: step < S)
       tc::wgmma_wait<0>();
-      if (s == 0 && n > 0 && wq == 0 && lane == 0) tc::mbar_arrive(&empty[(n - 1) % S]);
+      if (s == 0 && n > n0 && wq == 0 && lane == 0) tc::mbar_arrive(&empty[(n - step) % S]);
       float xv[kWgRows / 16][2][2];
 #pragma unroll
       for (int ks = 0; ks < kWgRows / 16; ++ks)
@@ -785,24 +820,23 @@ __global__ void __launch_bounds__(256, 1) cin_wg_wgrad_kernel(const __grid_const
       }
       tc::wgmma_commit();
     }
-    // refill the stage of block n - 1 with block n + S - 1 once every working warpgroup has released it
-    if (warp == 0) {
-      const int b = n + S - 1;
-      if (b < nb) {
-        if (b >= S) tc::mbar_wait(&empty[b % S], (b / S - 1) & 1);
-        issue(b);
-      }
-    }
   }
   tc::wgmma_wait<0>();
   tc::wgmma_fence_acc(acc[0]);
   tc::wgmma_fence_acc(acc[1]);
+  // the thread's rows again, from a fresh read of its index: kept live through the loop they would not fit the
+  // register budget at NP = 128
+  int lane_e;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(lane_e));
+  const int wq_e = (lane_e >> 5) & 3;
+  lane_e &= 31;
+  const int jw_e = (wq_e - 2 * (p.fields_per_tile == 2 && wq_e >= 2)) * 16 + (lane_e >> 2);
 #pragma unroll
   for (int s = 0; s < 2; ++s) {
     if (!tile_on[s]) continue;
 #pragma unroll
     for (int q = 0; q < NP / 2; ++q) {
-      const int r = (q >> 1) & 1, j = jw + 8 * r, l = 8 * (q >> 2) + c2 + (q & 1);
+      const int r = (q >> 1) & 1, j = jw_e + 8 * r, l = 8 * (q >> 2) + 2 * (lane_e & 3) + (q & 1);
       if (row_ok[s][r] && l < p.L && acc[s][q] != 0.f)
         atomicAdd(p.dw + ((int64_t)field[s] * H + j) * p.L + l, acc[s][q]);
     }
@@ -940,12 +974,64 @@ static int cin_wg_dgrad_launch(const CinWgBwdParams& p, cudaStream_t st) {
 }
 
 template <int NP>
-static int cin_wg_wgrad_launch(const CinWgWgradParams& p, int n_groups, int n_splits, cudaStream_t st) {
+static int cin_wg_wgrad_launch(const CinWgWgradParams& p, int n_ctas, cudaStream_t st) {
   const int smem = cin_wg_wgrad_layout(NP, p.F, p.h ? p.hpitch : 0, p.stages).total;
   DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_wgrad_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  cin_wg_wgrad_kernel<NP><<<dim3(n_groups, n_splits), 256, smem, st>>>(p);
+  // setmaxnreg only redistributes the registers the CTA got at launch: a smaller allocation would block the consumers
+  cudaFuncAttributes fa;
+  DTB_CUDA_OK(cudaFuncGetAttributes(&fa, cin_wg_wgrad_kernel<NP>));
+  if (fa.numRegs * kWgradThreads < 2 * 128 * kWgradConsumerRegs + 128 * kWgradProducerRegs) {
+    set_error("dtb_cin_bwd: the CIN weight-gradient kernel was built with too few registers for its warpgroup split");
+    return DTB_ERR_CUDA;
+  }
+  cin_wg_wgrad_kernel<NP><<<n_ctas, kWgradThreads, smem, st>>>(p);
   DTB_LAUNCH_OK();
   return DTB_OK;
+}
+
+// cuTensorMapEncodeTiled from the driver the runtime already loaded (no link against libcuda)
+static PFN_cuTensorMapEncodeTiled_v12000 cin_wg_tmap_encoder() {
+  static const PFN_cuTensorMapEncodeTiled_v12000 fn = [] {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &f, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      f = nullptr;
+    return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
+  }();
+  return fn;
+}
+
+// row splits of the weight gradient's field groups.  A full group's CTA costs 1 per row block.  With last_pair the
+// last group's CTA runs two blocks at a time, so it costs 1/2 per block and gets the SMs the full groups leave over.
+static void cin_wg_wgrad_grid(CinWgWgradParams& w, int64_t n_blocks, int sms) {
+  auto fit = [&](int64_t splits, int& s, int& bps) {      // at most n_blocks splits, none of them empty
+    splits = splits < 1 ? 1 : (splits > n_blocks ? n_blocks : splits);
+    bps = (int)((n_blocks + splits - 1) / splits);
+    s = (int)((n_blocks + bps - 1) / bps);
+  };
+  const int nfull = w.groups - 1;
+  if (!w.last_pair) {
+    fit(sms / w.groups, w.splits, w.blocks_per_split);
+    w.last_splits = w.splits; w.last_blocks_per_split = w.blocks_per_split;
+    return;
+  }
+  if (nfull == 0) {
+    w.splits = w.blocks_per_split = 0;
+    fit(sms, w.last_splits, w.last_blocks_per_split);
+    return;
+  }
+  int64_t best = -1;
+  for (int sf = 1; sf * nfull < sms; ++sf) {
+    int s, bps, sl, bpsl;
+    fit(sf, s, bps);
+    fit(sms - sf * nfull, sl, bpsl);
+    const int64_t cost = bps > (bpsl + 1) / 2 ? bps : (bpsl + 1) / 2;
+    if (best < 0 || cost < best) {
+      best = cost;
+      w.splits = s; w.blocks_per_split = bps; w.last_splits = sl; w.last_blocks_per_split = bpsl;
+    }
+  }
 }
 
 int cin_wg_bwd(const CinShape& s, const int32_t* idx, const int64_t* row_offsets, const float* weights,
@@ -1003,30 +1089,40 @@ int cin_wg_bwd(const CinShape& s, const int32_t* idx, const int64_t* row_offsets
       w.dc = dc + dc_off[k]; w.dw = d_weights + s.w_off[k];
       w.BD = BD; w.F = s.F; w.H = s.H[k]; w.L = s.L[k];
       w.fields_per_tile = s.H[k] <= 32 ? 2 : 1;
-      // rows of T_{k-1} start 16-byte aligned when ldh % 4 == 0: copy only their first H columns, to a pitch that makes
-      // the A-fragment reads free of bank conflicts (pitch % 16 in {4, 12}); otherwise copy the whole block
-      if (k > 0 && w.ldh % 4 == 0) {
+      // T_{k-1} is a tensor with 16-byte row strides when ldh % 4 == 0: one tensor copy per block brings the first
+      // hpitch >= H columns of its 64 rows, landing at a pitch that makes the A-fragment reads free of bank conflicts
+      // (pitch % 16 in {4, 12}); otherwise one bulk copy brings the whole rows
+      w.htensor = k > 0 && w.ldh % 4 == 0 && BD <= INT32_MAX;
+      if (w.htensor) {
         const int h4 = (s.H[k] + 3) / 4 * 4;
-        w.hrow_bytes = h4 * 4;
         w.hpitch = h4 + (20 - h4 % 16) % 16;
+        PFN_cuTensorMapEncodeTiled_v12000 encode = cin_wg_tmap_encoder();
+        const cuuint64_t dims[2] = {(cuuint64_t)w.ldh, (cuuint64_t)BD};
+        const cuuint64_t strides[1] = {(cuuint64_t)w.ldh * sizeof(float)};
+        const cuuint32_t box[2] = {(cuuint32_t)w.hpitch, (cuuint32_t)kWgRows}, estrides[2] = {1, 1};
+        if (!encode || encode(&w.hmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(w.h), dims, strides, box,
+                              estrides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
+          set_error("dtb_cin_bwd: cannot encode the tensor map of the CIN weight gradient's h rows");
+          return DTB_ERR_CUDA;
+        }
       } else {
-        w.hrow_bytes = 0;
         w.hpitch = w.ldh;
       }
       w.stages = cin_wg_wgrad_stages(np, s.F, w.h ? w.hpitch : 0);
       const int a_tiles = (s.F + w.fields_per_tile - 1) / w.fields_per_tile;
-      const int groups = (a_tiles + kWgradTiles - 1) / kWgradTiles;
-      int64_t splits = (int64_t)sm_count() / groups;
-      if (splits < 1) splits = 1;
-      if (splits > n_blocks) splits = n_blocks;
-      w.blocks_per_split = (int)((n_blocks + splits - 1) / splits);
-      splits = (n_blocks + w.blocks_per_split - 1) / w.blocks_per_split;
+      w.groups = (a_tiles + kWgradTiles - 1) / kWgradTiles;
+      // a last group with tiles for one warpgroup shares them between both; a warpgroup keeps up to two blocks of
+      // the ring until it releases the older one, so the other needs at least one more stage
+      w.last_pair = a_tiles - (w.groups - 1) * kWgradTiles <= 2 && w.stages >= 3;
+      cin_wg_wgrad_grid(w, n_blocks, sm_count());
+      const int ctas = (w.groups - 1) * w.splits + w.last_splits;
       int rc;
       switch (np) {
-        case 16: rc = cin_wg_wgrad_launch<16>(w, groups, (int)splits, st); break;
-        case 32: rc = cin_wg_wgrad_launch<32>(w, groups, (int)splits, st); break;
-        case 64: rc = cin_wg_wgrad_launch<64>(w, groups, (int)splits, st); break;
-        default: rc = cin_wg_wgrad_launch<128>(w, groups, (int)splits, st); break;
+        case 16: rc = cin_wg_wgrad_launch<16>(w, ctas, st); break;
+        case 32: rc = cin_wg_wgrad_launch<32>(w, ctas, st); break;
+        case 64: rc = cin_wg_wgrad_launch<64>(w, ctas, st); break;
+        default: rc = cin_wg_wgrad_launch<128>(w, ctas, st); break;
       }
       if (rc != DTB_OK) return rc;
     }

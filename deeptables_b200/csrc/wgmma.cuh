@@ -1,4 +1,4 @@
-// Thin inline-PTX layer over the sm_90a tensor-core path: mbarrier, bulk async copy (TMA engine, non-tensor form),
+// Thin inline-PTX layer over the sm_90a tensor-core path: mbarrier, bulk async copy (TMA engine, plain and 2-D tensor),
 // warpgroup MMA (wgmma.mma_async, fp32 accumulators in registers) and its shared-memory matrix descriptor.
 // Bit layouts follow the PTX ISA "warpgroup-level matrix shared memory layout / matrix descriptor" sections.
 #pragma once
@@ -52,6 +52,21 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
       "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
+// tensor form, 2-D: the box at (c0 = column, c1 = row) of the tensor map, packed densely (box width = row pitch);
+// elements outside the tensor arrive as zeros and the whole box counts towards the transaction bytes
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+      : "memory");
+}
+
+// ---- per-warpgroup register budget (all warps of the warpgroup execute it) ------------------------
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ---- wgmma ------------------------------------------------------------------------------------
 // shared-memory matrix descriptor, K-major, no swizzle ("interleaved" 8x16B core matrices):

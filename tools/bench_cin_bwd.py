@@ -6,7 +6,8 @@ dtb_cin_bwd_phase calls with L2 flushed before each backward, as bench.py does.
 
 Prints ms per kernel and TFLOP/s per kernel: executed (what the tensor cores run: padded tiles, bf16x3 = 3 passes) and
 algorithmic (the FMAs of the math alone), both counted from the shape below, plus the card name and power limit.
-For the data gradient it also prints the bytes of weight chunks copied into shared memory and their rate.
+For the data gradient it also prints the bytes of weight chunks copied into shared memory and their rate; for each
+weight-gradient layer, the microseconds per 64-row block of its busiest CTA and the bytes bulk-copied per block.
 """
 import argparse
 import ctypes
@@ -41,6 +42,67 @@ def dgrad_chunks(b):
     return nch, nbytes, n_blocks
 
 
+def wgrad_plan(b, sms, f=F, d=D, sizes=SIZES):
+    """Per layer, the launch of cin_wg_wgrad_kernel as csrc/cin_wgmma.cu plans it: field groups of four m64 A tiles,
+    the h copy, the ring depth, the row splits and the bytes bulk-copied per 64-row block."""
+    from oracle import layers_ref as L
+    bd = b * d
+    n_blocks = (bd + 63) // 64
+    H = L.cin_field_nums(f, sizes, False)[:len(sizes)]
+    np_ = 16
+    while np_ < max(sizes):
+        np_ *= 2
+    r128 = lambda x: (x + 127) // 128 * 128
+
+    def fit(splits):
+        splits = min(max(splits, 1), n_blocks)
+        bps = -(-n_blocks // splits)
+        return -(-n_blocks // bps), bps
+
+    plans = []
+    for k, h in enumerate(H):
+        ldh = f if k == 0 else sizes[k - 1]
+        fpt = 2 if h <= 32 else 1
+        htensor = k > 0 and ldh % 4 == 0
+        if htensor:
+            h4 = (h + 3) // 4 * 4
+            hpitch = h4 + (20 - h4 % 16) % 16
+        else:
+            hpitch = ldh if k > 0 else 0
+        stage = r128(np_ * 64 * 4 + r128(64 * f * 4)) if hpitch == 0 else np_ * 64 * 4 + r128(64 * f * 4) + r128(64 * hpitch * 4)
+        stages = 4
+        while stages > 2 and stages * stage + 16 * stages > 227 * 1024:
+            stages -= 1
+        a_tiles = -(-f // fpt)
+        groups = -(-a_tiles // 4)
+        pair = a_tiles - 4 * (groups - 1) <= 2 and stages >= 3
+        if not pair:
+            sf, bps = fit(sms // groups)
+            sl, bpsl = sf, bps
+        elif groups == 1:
+            sf, bps = 0, 0
+            sl, bpsl = fit(sms)
+        else:
+            best = None
+            for s in range(1, sms):
+                if s * (groups - 1) >= sms:
+                    break
+                a, ab = fit(s)
+                c, cb = fit(sms - s * (groups - 1))
+                cost = max(ab, (cb + 1) // 2)
+                if best is None or cost < best[0]:
+                    best = (cost, a, ab, c, cb)
+            _, sf, bps, sl, bpsl = best
+        copied = np_ * 64 * 4 + 64 * f * 4 + (0 if k == 0 else 64 * hpitch * 4 if htensor else 64 * ldh * 4)
+        # blocks the busiest CTA multiplies with each warpgroup (a paired last group splits its blocks in two)
+        crit = max(bps, (bpsl + 1) // 2 if pair else bpsl)
+        plans.append(dict(fields_per_tile=fpt, a_tiles=a_tiles, groups=groups, htensor=htensor, hpitch=hpitch,
+                          stages=stages, last_pair=pair, splits=sf, blocks_per_split=bps, last_splits=sl,
+                          last_blocks_per_split=bpsl, ctas=(groups - 1) * sf + sl, bytes_per_block=copied,
+                          critical_blocks=crit))
+    return plans
+
+
 def flop_counts(b):
     """FMA counts per kernel: {name: (executed, algorithmic)}; mirrors the tiling of csrc/cin_wgmma.cu."""
     bd, n_blocks, H, npj = _shape(b)
@@ -55,8 +117,10 @@ def flop_counts(b):
         fpt = 2 if h <= 32 else 1
         a_tiles = (F + fpt - 1) // fpt
         groups = (a_tiles + 3) // 4
-        # every working warpgroup runs both of its tiles (an absent one on zero rows)
-        tiles = sum(2 for g in range(groups) for w in range(2) if (4 * g + 2 * w) * fpt < F)
+        # each block is multiplied by all four tiles of a full field group, and by the two tiles of a last group that
+        # has tiles for one warpgroup only (whether one warpgroup runs them or both do, on alternate blocks); an
+        # absent tile past the last field runs on zero rows
+        tiles = 4 * (groups - 1) + (4 if a_tiles - 4 * (groups - 1) > 2 else 2)
         out[f'cin_wg_wgrad_kernel layer {k}'] = (tiles * 64 * np_ * n_blocks * 64 * 3, bd * F * h * s)
     return out
 
@@ -135,6 +199,7 @@ def main():
             continue
         times.setdefault(key, []).append(e.time_range.elapsed_us() * 1e-3)
     flops = flop_counts(b)
+    plans = wgrad_plan(b, torch.cuda.get_device_properties(0).multi_processor_count)
     res = {'gpu': gpu_info(), 'batch': b, 'gemm_rows': b * D, 'iters': args.iters, 'kernels': {}}
     wg_total = 0.0
     for key, (exe, alg) in flops.items():
@@ -144,8 +209,13 @@ def main():
         ms = ts[len(ts) // 2]
         if key.startswith('cin_wg_wgrad'):
             wg_total += ms
-        res['kernels'][key] = {'ms': round(ms, 4), 'executed_tflops': round(2 * exe / ms * 1e-9, 1),
-                               'algorithmic_tflops': round(2 * alg / ms * 1e-9, 1)}
+            # time per 64-row block of the busiest CTA, and what one block brings into shared memory
+            pl = plans[int(key.rsplit(' ', 1)[1])]
+            res['kernels'].setdefault(key, {}).update(
+                us_per_block_per_cta=round(ms * 1e3 / pl['critical_blocks'], 3), bytes_per_block=pl['bytes_per_block'],
+                ctas=pl['ctas'], h_copy='tensor' if pl['htensor'] else ('rows' if pl['hpitch'] else 'none'))
+        res['kernels'].setdefault(key, {}).update(ms=round(ms, 4), executed_tflops=round(2 * exe / ms * 1e-9, 1),
+                                                  algorithmic_tflops=round(2 * alg / ms * 1e-9, 1))
         if key == 'cin_wg_dgrad_kernel':
             # weight chunks bulk-copied from L2 into shared memory, one copy per tile and chunk
             _, tile_bytes, n_tiles = dgrad_chunks(b)
