@@ -242,7 +242,7 @@ class CIN(Layer):
         self.direct = params.get('direct', False)
         self.reduce_D = params.get('reduce_D', False)
         # test hook: DTB_CIN_PRECISION overrides the auto choice (0) so the whole GPU suite can be run on another CIN mode
-        self.precision = params.get('precision', 0) or int(os.environ.get('DTB_CIN_PRECISION', 0))   # engine knob: 0 auto (fp16 single pass where supported, else bf16x3), 1 any-shape, 2 bf16x3, 3 bf16x1, 4 fp16x1
+        self.precision = params.get('precision', 0) or int(os.environ.get('DTB_CIN_PRECISION', 0))   # engine knob: 0 auto (fused bf16x3 where supported, else any-shape), 1 any-shape, 2 bf16x3, 3 bf16x1, 4 fp16x1
         if len(self.cross_layer_size) == 0:
             raise ValueError('cross_layer_size must be a list(tuple) of length greater than 1')
         if self.activation not in E.ACT_CODES:
