@@ -6,13 +6,16 @@
 // register layout wgmma expects for an A operand -- so layer k's output feeds layer k+1 without leaving the registers.
 // Per x0 field i the thread scales its h fragment by x0[m,i] and issues wgmma with A from registers; the weight chunk
 // of field i (all hidden fields x all feature maps, pre-packed as K-major bf16/fp16 core matrices) arrives in shared
-// memory by one bulk async copy, double-buffered.
+// memory by one bulk async copy.  A forward CTA (one per SM) runs two such warpgroups on a pair of adjacent tiles, so
+// each chunk is copied once per 128 rows, into a ring of full/empty mbarrier stages; a third, producer warpgroup owns
+// the copies, gathers the next pair's x0 rows, and stores each finished layer's saved rows and pooled sums from a
+// shared-memory staging tile while the consumers go on to the next layer.
 //
 // Precision: 2 = bf16x3 split (Z_hi W_hi + Z_lo W_hi + Z_hi W_lo: fp32-grade), 3 = one bf16 pass, 4 = one fp16 pass on
 // operands scaled by exact powers of two (per GEMM row for Z, per layer for W_k), undone on the fp32 accumulator.
 // The saved activations have the layout of the any-shape formulation (x0t, then T_k).  The backward (below) runs the
 // data and weight gradients as two fused wgmma kernels in bf16x3 for every precision code.  The data-gradient kernel
-// (one warpgroup per CTA, like the forward; one W_k^T chunk serves two x0 fields where 2 H_k <= NPJ) hands dC_k to the
+// (one warpgroup per CTA; one W_k^T chunk serves two x0 fields where 2 H_k <= NPJ) hands dC_k to the
 // weight-gradient kernel already split into the bf16 hi/lo image wgmma reads; the weight-gradient CTA is two
 // warpgroups that share each copied 64-row block among four m64 A tiles (one or two x0 fields each), fed by a
 // multi-stage ring that a third, producer warpgroup refills.
@@ -22,6 +25,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cudaTypedefs.h>      // CUtensorMap, PFN_cuTensorMapEncodeTiled
+#include <type_traits>
 
 namespace dtb {
 
@@ -42,6 +46,8 @@ struct CinWgParams {
   int* status;
   const int* wmax;       // fp16: bit pattern of max|W_k| per layer
   int B, D, F, n_layers, act, P;
+  int n_tiles;           // 64-row tiles: ceil(B * D / 64)
+  int hp_max, stages;    // the widest layer's padded hidden fields; weight-chunk stages in shared memory
   int L[kCinMaxLayers], Hp[kCinMaxLayers], hid_n[kCinMaxLayers];
   int pool_lo[kCinMaxLayers], pool_n[kCinMaxLayers], pcol0[kCinMaxLayers];
   unsigned long long wpack_off[kCinMaxLayers], saved_off[kCinMaxLayers], bias_off[kCinMaxLayers];
@@ -89,21 +95,39 @@ __global__ void cin_wg_wmax_kernel(const float* __restrict__ w, int64_t n, int* 
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_int(m));    // non-negative floats order as ints
 }
 
+// Forward CTA: consumer warpgroups 0 and 1 each own one 64-row tile of a pair of adjacent tiles (128 GEMM rows) and
+// share every weight chunk copied for the pair; producer warpgroup 2 brings the chunks into a ring of full/empty
+// mbarrier stages (thread 0 of its first warp), gathers the x0 rows of the next pair into the other of two x0 slots
+// and takes each finished layer's tile from the consumers' staging buffers to the saved T_k rows and the pooled sums
+// (its other three warps).  One CTA per SM runs pairs blockIdx.x, blockIdx.x + gridDim.x, ...
+constexpr int kFwdThreads = 384;
+constexpr int kFwdMaxStages = 8;
+constexpr int kFwdAux = 96;             // producer threads that gather x0 and store the epilogues (warps 1-3 of it)
+// the registers the CTA gets at launch (384 x 168) are shared out again: 2 x 128 x 216 + 128 x 72 = 384 x 168
+constexpr int kFwdConsumerRegs = 216, kFwdProducerRegs = 72;
+
 struct CinWgSmem {
-  int w_off, x0_off, out_off, bar_off, total;
+  int stage, x0_off, ot_off, bar_off, total;
 };
-__host__ __device__ inline CinWgSmem cin_wg_layout(int NP, int F, int mode) {
+// stages x weight chunks of the widest layer (hp_max), two x0 slots of 128 rows, one staging tile per consumer, and
+// the mbarriers: full/empty per stage, x0 full per slot, staging full/empty per consumer
+__host__ __device__ inline CinWgSmem cin_wg_layout(int NP, int F, int mode, int hp_max, int stages) {
   CinWgSmem l;
-  const int wbuf = (int)cin_wg_chunk_bytes(NP, kWgMaxHp, mode);
-  l.w_off = 0;
-  l.x0_off = 2 * wbuf;
-  l.out_off = l.x0_off + kWgRows * F * 4;
-  l.bar_off = (l.out_off + kWgRows * (NP + 1) * 4 + 15) / 16 * 16;
-  l.total = l.bar_off + 16;
+  l.stage = (int)cin_wg_chunk_bytes(NP, hp_max, mode);
+  l.x0_off = stages * l.stage;
+  l.ot_off = l.x0_off + (2 * 2 * kWgRows * F * 4 + 127) / 128 * 128;
+  l.bar_off = l.ot_off + 2 * kWgRows * (NP + 1) * 4;
+  l.total = l.bar_off + 8 * (2 * stages + 2 + 4);
   return l;
 }
+// as many stages as fit in shared memory, 2 to kFwdMaxStages (0: not even 2 fit)
+static int cin_wg_fwd_stages(int NP, int F, int mode, int hp_max) {
+  int s = kFwdMaxStages;
+  while (s >= 2 && cin_wg_layout(NP, F, mode, hp_max, s).total > 227 * 1024) --s;
+  return s >= 2 ? s : 0;
+}
 
-// weight chunk number c of this CTA's schedule (tiles x layers x fields) -> source and size
+// weight chunk of layer k, x0 field i -> source and size
 __device__ __forceinline__ void cin_wg_chunk_src(const CinWgParams& p, int NP, int mode, int k, int i, const uint8_t*& src,
                                                  uint32_t& bytes) {
   bytes = cin_wg_chunk_bytes(NP, p.Hp[k], mode);
@@ -111,55 +135,143 @@ __device__ __forceinline__ void cin_wg_chunk_src(const CinWgParams& p, int NP, i
 }
 
 template <int NP, int kMode>
-__global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__ CinWgParams p) {
+__global__ void __launch_bounds__(kFwdThreads, 1) cin_wg_fwd_kernel(const __grid_constant__ CinWgParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
-  const CinWgSmem lay = cin_wg_layout(NP, p.F, kMode);
-  const uint32_t wbuf_bytes = cin_wg_chunk_bytes(NP, kWgMaxHp, kMode);
-  uint8_t* wbuf = smem + lay.w_off;
-  float* x0s = reinterpret_cast<float*>(smem + lay.x0_off);      // [m][i]
-  float* ot = reinterpret_cast<float*>(smem + lay.out_off);      // [m][NP + 1]
+  const int S = p.stages;
+  const CinWgSmem lay = cin_wg_layout(NP, p.F, kMode, p.hp_max, S);
+  float* x0buf = reinterpret_cast<float*>(smem + lay.x0_off);    // slot s: [128 rows][F]
+  float* otbuf = reinterpret_cast<float*>(smem + lay.ot_off);    // consumer w: [64 rows][NP + 1]
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint64_t* empty = full + S;
+  uint64_t* x0_full = empty + S;
+  uint64_t* ot_full = x0_full + 2;
+  uint64_t* ot_empty = ot_full + 2;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
   const int F = p.F, D = p.D;
   const int64_t BD = (int64_t)p.B * D;
-  const int n_tiles = (int)((BD + kWgRows - 1) / kWgRows);
-  const int r0 = warp * 16 + (lane >> 2), c2 = 2 * (lane & 3);    // accumulator rows r0, r0 + 8; column pair base
-  constexpr uint32_t lbo_b = (NP >> 3) * 128;
+  const int n_tiles = p.n_tiles, n_pairs = (p.n_tiles + 1) / 2;      // from the parameters: reloaded, not spilled
 
   if (tid == 0) {
-    tc::mbar_init(&full[0], 1);
-    tc::mbar_init(&full[1], 1);
+    for (int s = 0; s < S; ++s) {
+      tc::mbar_init(&full[s], 1);
+      tc::mbar_init(&empty[s], 8);      // each warp of both consumers; a consumer alone in a pair arrives twice
+    }
+    for (int s = 0; s < 2; ++s) {
+      tc::mbar_init(&x0_full[s], kFwdAux);
+      tc::mbar_init(&ot_full[s], 128);
+      tc::mbar_init(&ot_empty[s], kFwdAux);
+    }
     tc::fence_barrier_init();
   }
   __syncthreads();
-  // the copy of chunk c goes to buffer c & 1; it is issued while chunk c - 1 is multiplied
-  auto issue = [&](uint32_t c, int k, int i) {
-    const uint8_t* src;
-    uint32_t bytes;
-    cin_wg_chunk_src(p, NP, kMode, k, i, src, bytes);
-    tc::mbar_arrive_expect_tx(&full[c & 1], bytes);
-    tc::bulk_g2s(wbuf + (c & 1) * wbuf_bytes, src, bytes, &full[c & 1]);
-  };
-  if (tid == 0 && (int)blockIdx.x < n_tiles) issue(0, 0, 0);
 
-  uint32_t chunk = 0;
-  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int64_t gm0 = (int64_t)tile * kWgRows;
-    // ---- x0 block of the 64 rows (m fastest: consecutive threads read consecutive floats of one embedding row)
-    for (int e = tid; e < kWgRows * F; e += 128) {
-      const int i = e / kWgRows, m = e - i * kWgRows;
-      const int64_t gm = gm0 + m;
-      float v = 0.f;
-      if (gm < BD) {
-        const int64_t b = gm / D;
-        const int d = (int)(gm - b * D);
-        const int64_t rb = table_row(p.row_offsets, i, __ldg(p.idx + b * F + i), D, p.status);
-        if (rb >= 0) v = __ldg(p.table + rb + d);
-        if (p.saved) p.saved[gm * F + i] = v;
+  if (wg == 2) {
+    tc::setmaxnreg_dec<kFwdProducerRegs>();
+    const int pt = tid - 2 * 128;
+    if (pt == 0) {
+      // weight chunks: pair x layer x field, chunk c into stage c % S once both consumers released chunk c - S
+      int st = 0;
+      uint32_t ph = 0, c = 0;
+      for (int pr = blockIdx.x; pr < n_pairs; pr += gridDim.x)
+        for (int k = 0; k < p.n_layers; ++k)
+          for (int i = 0; i < F; ++i, ++c) {
+            const uint8_t* src;
+            uint32_t bytes;
+            cin_wg_chunk_src(p, NP, kMode, k, i, src, bytes);
+            if (c >= (uint32_t)S) tc::mbar_wait(&empty[st], ph ^ 1);
+            tc::mbar_arrive_expect_tx(&full[st], bytes);
+            tc::bulk_g2s(smem + st * lay.stage, src, bytes, &full[st]);
+            if (++st == S) { st = 0; ph ^= 1; }
+          }
+    } else if (pt >= 32) {
+      const int gt = pt - 32, gw = gt >> 5;
+      const int lgD = __ffs(D) - 1;      // D is a power of two
+      // x0 rows of pair pr into slot s (m fastest: consecutive threads read consecutive floats of one embedding row),
+      // then the pair's x0t block, contiguous in saved, from shared memory
+      auto gather = [&](int pr, int s) {
+        float* xs = x0buf + s * 2 * kWgRows * F;
+        const int64_t gm0 = (int64_t)pr * 2 * kWgRows;
+        const int n = 2 * kWgRows * F;
+        constexpr int U = 4;      // independent id -> row -> value chains in flight per thread
+        for (int e0 = gt; e0 < n; e0 += kFwdAux * U) {
+          int64_t rb[U];
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            const int e = e0 + u * kFwdAux, i = e >> 7;
+            const int64_t gm = gm0 + (e & 127), b = gm >> lgD;
+            rb[u] = -1;
+            if (e < n && gm < BD) {
+              rb[u] = table_row(p.row_offsets, i, __ldg(p.idx + b * F + i), D, p.status);
+              if (rb[u] >= 0) rb[u] += gm & (D - 1);
+            }
+          }
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            const int e = e0 + u * kFwdAux;
+            if (e < n) xs[(e & 127) * F + (e >> 7)] = rb[u] >= 0 ? __ldg(p.table + rb[u]) : 0.f;
+          }
+        }
+        tc::named_bar_sync(1, kFwdAux);
+        tc::mbar_arrive(&x0_full[s]);
+        if (p.saved) {
+          const int rows = BD - gm0 < 2 * kWgRows ? (int)(BD - gm0) : 2 * kWgRows;
+          for (int e = gt; e < rows * F; e += kFwdAux) p.saved[gm0 * F + e] = xs[e];
+        }
+      };
+      uint32_t ot_ph = 0;      // bit w: phase of consumer w's staging-full barrier
+      int jj = 0;
+      if ((int)blockIdx.x < n_pairs) gather(blockIdx.x, 0);
+      // the next pair's x0 goes in after this pair's layer-0 tiles are stored (before them with one layer): a
+      // consumer waits for the store of layer k at the end of layer k + 1, and layers 1 and more are the long ones
+      const int k_gather = p.n_layers > 1 ? 1 : 0;
+      for (int pr = blockIdx.x; pr < n_pairs; pr += gridDim.x, ++jj) {
+        const int nw = 2 * pr + 1 < n_tiles ? 2 : 1;
+        for (int k = 0; k < p.n_layers; ++k) {
+          // slot (jj + 1) & 1 held pair jj - 1, whose last layer both consumers have handed over: its x0 is read
+          if (k == k_gather && pr + (int)gridDim.x < n_pairs) gather(pr + gridDim.x, (jj + 1) & 1);
+          const int L = p.L[k], rows_b = kWgRows / D, pool_n = p.pool_n[k];
+          for (int w = 0; w < nw; ++w) {
+            const float* ot = otbuf + w * kWgRows * (NP + 1);
+            const int64_t gm0 = (int64_t)(2 * pr + w) * kWgRows;
+            tc::mbar_wait(&ot_full[w], (ot_ph >> w) & 1);
+            ot_ph ^= 1u << w;
+            if (p.saved) {
+              float* T = p.saved + p.saved_off[k];
+              for (int m = gw; m < kWgRows; m += kFwdAux / 32)
+                if (gm0 + m < BD)
+                  for (int col = lane; col < L; col += 32) T[(gm0 + m) * L + col] = ot[m * (NP + 1) + col];
+            }
+            for (int e = gt; e < rows_b * pool_n; e += kFwdAux) {
+              const int bl = e / pool_n, q = e - bl * pool_n;
+              const int64_t b = gm0 / D + bl;
+              if (b < p.B) {
+                float sum = 0.f;
+                for (int d = 0; d < D; ++d) sum += ot[(bl * D + d) * (NP + 1) + p.pool_lo[k] + q];
+                p.pooled[b * p.P + p.pcol0[k] + q] = sum;
+              }
+            }
+            tc::mbar_arrive(&ot_empty[w]);
+          }
+        }
       }
-      x0s[m * F + i] = v;
     }
-    __syncthreads();
+    return;
+  }
+  tc::setmaxnreg_inc<kFwdConsumerRegs>();
+
+  // consumers
+  const int r0 = wq * 16 + (lane >> 2), c2 = 2 * (lane & 3);    // accumulator rows r0, r0 + 8; column pair base
+  constexpr uint32_t lbo_b = (NP >> 3) * 128;
+  constexpr bool kTwoSets = kMode != 0;      // A-fragment sets: one wgmma group in flight while the next is built
+  float* ot = otbuf + wg * kWgRows * (NP + 1);
+  int st = 0, ep = 0;
+  uint32_t ph = 0;
+  int jj = 0;
+  for (int pr = blockIdx.x; pr < n_pairs; pr += gridDim.x, ++jj) {
+    if (2 * pr + wg >= n_tiles) break;      // the last pair of an odd tile count: warpgroup 1 has no tile
+    const uint32_t rel = 2 * pr + 1 < n_tiles ? 1u : 2u;      // empty-barrier arrivals per warp
+    const float* x0s = x0buf + ((jj & 1) * 2 + wg) * kWgRows * F;      // [m][i]
+    tc::mbar_wait(&x0_full[jj & 1], (jj >> 1) & 1);
     // h_0 = x0, in accumulator fragment order: hh[q] = h[row r0 + 8*((q>>1)&1), col 8*(q>>2) + c2 + (q&1)]
     float hh[kWgMaxHp / 2];
 #pragma unroll
@@ -167,17 +279,18 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
       const int row = r0 + (((q >> 1) & 1) << 3), col = 8 * (q >> 2) + c2 + (q & 1);
       hh[q] = col < F ? x0s[row * F + col] : 0.f;
     }
-    [[maybe_unused]] float xmax[2] = {0.f, 0.f};
-    if constexpr (kMode == 2) {
-      for (int i = 0; i < F; ++i) {
-        xmax[0] = fmaxf(xmax[0], fabsf(x0s[r0 * F + i]));
-        xmax[1] = fmaxf(xmax[1], fabsf(x0s[(r0 + 8) * F + i]));
-      }
-    }
     for (int k = 0; k < p.n_layers; ++k) {
       const int Hp = p.Hp[k], L = p.L[k];
+      // fp16: srow scales the thread's two Z rows into range, inv_acc undoes it and the weight scale on the
+      // accumulator.  Both come from x0, h and max|W_k| alone, so inv_acc is worked out again for the epilogue
+      // rather than held through the MMAs (hh does not change in between).
       [[maybe_unused]] float srow[2] = {1.f, 1.f}, inv_acc[2] = {1.f, 1.f};
-      if constexpr (kMode == 2) {
+      auto fp16_scales = [&]() {
+        float xmax[2] = {0.f, 0.f};
+        for (int i = 0; i < F; ++i) {
+          xmax[0] = fmaxf(xmax[0], fabsf(x0s[r0 * F + i]));
+          xmax[1] = fmaxf(xmax[1], fabsf(x0s[(r0 + 8) * F + i]));
+        }
         float sw, inv_w;
         tc::pow2_scale_to_1024(__int_as_float(__ldg(p.wmax + k)), sw, inv_w);
 #pragma unroll
@@ -192,43 +305,43 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
           tc::pow2_scale_to_1024(xmax[h] * m, srow[h], inv_row);
           inv_acc[h] = inv_row * inv_w;
         }
-      }
+      };
+      if constexpr (kMode == 2) fp16_scales();
       float acc[NP / 2];
 #pragma unroll
       for (int q = 0; q < NP / 2; ++q) acc[q] = 0.f;
-      for (int i = 0; i < F; ++i, ++chunk) {
-        // prefetch the next chunk of the schedule into the other buffer (its last reader finished: see the
-        // __syncthreads at the end of the previous iteration)
-        if (tid == 0) {
-          int nk = k, ni = i + 1;
-          bool more = true;
-          if (ni == F) {
-            ni = 0;
-            if (++nk == p.n_layers) { nk = 0; more = tile + (int)gridDim.x < n_tiles; }
+      // the layer's fields with KS = Hp / 16 k-steps known at compile time: a branch on Hp between wgmma groups in
+      // flight would make ptxas serialize every wgmma
+      auto run_layer = [&](auto ks_c) {
+        constexpr int KS = decltype(ks_c)::value;
+        // A fragments of field i: Z[m, kk] = x0[m, i] h[m, kk]
+        auto build = [&](uint32_t (&ahi)[KS][4], uint32_t (&alo)[KS][4], int i) {
+          float x[2] = {x0s[r0 * F + i], x0s[(r0 + 8) * F + i]};
+          if constexpr (kMode == 2) { x[0] *= srow[0]; x[1] *= srow[1]; }
+#pragma unroll
+          for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+            for (int f = 0; f < 4; ++f) {
+              const float xv = x[f & 1];
+              const float z0 = xv * hh[8 * ks + 2 * f], z1 = xv * hh[8 * ks + 2 * f + 1];
+              if constexpr (kMode == 0) tc::split_bf16x2(z0, z1, ahi[ks][f], alo[ks][f]);
+              else if constexpr (kMode == 1) ahi[ks][f] = tc::pack_bf16x2(z0, z1);
+              else ahi[ks][f] = tc::pack_f16x2(z0, z1);
+            }
           }
-          if (more) issue(chunk + 1, nk, ni);
-        }
-        float x[2] = {x0s[r0 * F + i], x0s[(r0 + 8) * F + i]};
-        if constexpr (kMode == 2) { x[0] *= srow[0]; x[1] *= srow[1]; }
-        uint32_t ahi[kWgMaxHp / 16][4], alo[kWgMaxHp / 16][4];
+        };
+        // field i: its MMAs on the chunk in stage st go out; once field i - 1's are done, its stage is released and
+        // the fragments of field i + 1 are built into the set field i - 1 used, while field i's MMAs run.  bf16x3
+        // has no registers for a second hi + lo set next to the accumulator (ptxas serializes the wgmma): it waits
+        // for field i's MMAs, releases their stage and builds into the same set, while the other consumer multiplies.
+        auto field = [&](uint32_t (&ahi)[KS][4], uint32_t (&alo)[KS][4], uint32_t (&nhi)[KS][4],
+                         uint32_t (&nlo)[KS][4], int i) {
+          tc::mbar_wait(&full[st], ph);
+          const uint32_t b_hi = tc::smem_u32(smem + st * lay.stage);
+          const uint32_t b_lo = b_hi + (uint32_t)NP * KS * 16 * 2;
+          tc::wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < kWgMaxHp / 16; ++ks) {
-#pragma unroll
-          for (int f = 0; f < 4; ++f) {
-            const float xv = x[f & 1];
-            const float z0 = xv * hh[8 * ks + 2 * f], z1 = xv * hh[8 * ks + 2 * f + 1];
-            if constexpr (kMode == 0) tc::split_bf16x2(z0, z1, ahi[ks][f], alo[ks][f]);
-            else if constexpr (kMode == 1) ahi[ks][f] = tc::pack_bf16x2(z0, z1);
-            else ahi[ks][f] = tc::pack_f16x2(z0, z1);
-          }
-        }
-        tc::mbar_wait(&full[chunk & 1], (chunk >> 1) & 1);
-        const uint32_t b_hi = tc::smem_u32(wbuf + (chunk & 1) * wbuf_bytes);
-        const uint32_t b_lo = b_hi + (uint32_t)NP * Hp * 2;
-        tc::wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < kWgMaxHp / 16; ++ks) {
-          if (ks * 16 < Hp) {
+          for (int ks = 0; ks < KS; ++ks) {
             const uint32_t first = (i == 0 && ks == 0) ? 0u : 1u;
             const uint64_t dh = tc::make_smem_desc(b_hi + ks * 2 * lbo_b, lbo_b, 128);
             if constexpr (kMode == 2) {
@@ -241,16 +354,45 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
               }
             }
           }
+          tc::wgmma_commit();
+          if constexpr (kTwoSets) {
+            tc::wgmma_wait<1>();
+            tc::mbar_arrive_if(&empty[st == 0 ? S - 1 : st - 1], rel, i > 0 && lane == 0);
+          } else {
+            tc::wgmma_wait<0>();
+            tc::mbar_arrive_if(&empty[st], rel, lane == 0);
+          }
+          if (++st == S) { st = 0; ph ^= 1; }
+          if (i + 1 < F) build(nhi, nlo, i + 1);
+        };
+        uint32_t ahi0[KS][4], alo0[KS][4], ahi1[KS][4], alo1[KS][4];
+        build(ahi0, alo0, 0);
+        for (int i = 0; i < F; i += 2) {
+          if constexpr (kTwoSets) {
+            field(ahi0, alo0, ahi1, alo1, i);
+            if (i + 1 < F) field(ahi1, alo1, ahi0, alo0, i + 1);
+          } else {
+            field(ahi0, alo0, ahi0, alo0, i);
+            if (i + 1 < F) field(ahi0, alo0, ahi0, alo0, i + 1);
+          }
         }
-        tc::wgmma_commit();
         tc::wgmma_wait<0>();
-        tc::wgmma_fence_acc(acc);
-        __syncthreads();
+      };
+      switch (Hp >> 4) {
+        case 1: run_layer(std::integral_constant<int, 1>{}); break;
+        case 2: run_layer(std::integral_constant<int, 2>{}); break;
+        case 3: run_layer(std::integral_constant<int, 3>{}); break;
+        default: run_layer(std::integral_constant<int, 4>{}); break;
       }
-      // ---- epilogue of layer k: bias / act in registers; the tile goes through shared memory for the coalesced saved
-      //      rows and the deterministic sum over d of the pooled feature maps
+      tc::wgmma_fence_acc(acc);
+      if constexpr (kTwoSets) tc::mbar_arrive_if(&empty[st == 0 ? S - 1 : st - 1], rel, lane == 0);
+      if constexpr (kMode == 2) fp16_scales();
+      // ---- epilogue of layer k: bias / act in registers, then the tile goes to the staging buffer once the producer
+      //      has taken the previous one; the producer stores the saved rows and the pooled sums from it
       const float* bias = p.bias ? p.bias + p.bias_off[k] : nullptr;
       const int hid_next = k + 1 < p.n_layers ? p.hid_n[k] : 0;
+      if (ep > 0) tc::mbar_wait(&ot_empty[wg], (ep - 1) & 1);
+      ++ep;
 #pragma unroll
       for (int q = 0; q < NP / 2; ++q) {
         const int h = (q >> 1) & 1;
@@ -262,32 +404,14 @@ __global__ void __launch_bounds__(128) cin_wg_fwd_kernel(const __grid_constant__
         if (col < L) ot[row * (NP + 1) + col] = v;
         if (q < kWgMaxHp / 2) hh[q] = col < hid_next ? v : 0.f;
       }
-      __syncthreads();
-      if (p.saved) {
-        float* T = p.saved + p.saved_off[k];
-        for (int e = tid; e < kWgRows * L; e += 128) {
-          const int m = e / L, col = e - m * L;
-          if (gm0 + m < BD) T[(gm0 + m) * L + col] = ot[m * (NP + 1) + col];
-        }
-      }
-      const int rows_b = kWgRows / D, pool_n = p.pool_n[k];
-      for (int e = tid; e < rows_b * pool_n; e += 128) {
-        const int bl = e / pool_n, q = e - bl * pool_n;
-        const int64_t b = gm0 / D + bl;
-        if (b < p.B) {
-          float sum = 0.f;
-          for (int d = 0; d < D; ++d) sum += ot[(bl * D + d) * (NP + 1) + p.pool_lo[k] + q];
-          p.pooled[b * p.P + p.pcol0[k] + q] = sum;
-        }
-      }
-      __syncthreads();
+      tc::mbar_arrive(&ot_full[wg]);
     }
   }
 }
 
 // ==========================================================================================
 // Backward (bf16x3 split, every precision code), two kernels:
-//   dgrad, per 64-row tile, layers last -> first (one warpgroup, like the forward):
+//   dgrad, per 64-row tile, layers last -> first (one warpgroup per CTA):
 //     dC_k = (d_pooled part + dh_{k+1}) * act'(T_k)                 registers, accumulator fragment layout
 //     dZ_{k,i}[m, j] = sum_l dC_k[m, l] W_k[i*H + j, l]             wgmma: A = dC_k from registers, B = W_k^T chunk
 //     dx0[m, i] += sum_j dZ h_k[m, j] ;  dh_k[m, j] += dZ x0[m, i]   registers (dh_k feeds dC_{k-1})
@@ -852,12 +976,18 @@ static int cin_wg_np(const CinShape& s) {
   return np;
 }
 
+static int cin_wg_hp_max(const CinShape& s) {
+  int hp = 16;
+  for (int k = 0; k < s.n_layers; ++k) hp = round_up16(s.H[k]) > hp ? round_up16(s.H[k]) : hp;
+  return hp;
+}
+
 bool cin_wg_supported(const CinShape& s) {
   if (!(s.D == 4 || s.D == 8 || s.D == 16 || s.D == 32)) return false;      // D divides the 64-row tile
   if (s.F < 1 || s.F > kWgMaxHp || s.Lmax > kWgMaxNP) return false;
   for (int k = 0; k < s.n_layers; ++k)
     if (round_up16(s.H[k]) > kWgMaxHp) return false;
-  return cin_wg_layout(cin_wg_np(s), s.F, 0).total <= 227 * 1024;
+  return cin_wg_fwd_stages(cin_wg_np(s), s.F, 0, cin_wg_hp_max(s)) >= 2;      // bf16x3 needs the most
 }
 
 size_t cin_wg_workspace_bytes(const CinShape& s) {
@@ -869,15 +999,18 @@ size_t cin_wg_workspace_bytes(const CinShape& s) {
 
 template <int NP, int kMode>
 static int cin_wg_launch(const CinWgParams& p, cudaStream_t st) {
-  const CinWgSmem lay = cin_wg_layout(NP, p.F, kMode);
-  DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_fwd_kernel<NP, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
-  const int64_t n_tiles = ((int64_t)p.B * p.D + kWgRows - 1) / kWgRows;
-  int per_sm = (227 * 1024) / (lay.total + 1024);
-  if (per_sm < 1) per_sm = 1;
-  if (per_sm > 4) per_sm = 4;
-  int64_t grid = (int64_t)sm_count() * per_sm;
-  if (grid > n_tiles) grid = n_tiles;
-  cin_wg_fwd_kernel<NP, kMode><<<(int)grid, 128, lay.total, st>>>(p);
+  const int smem = cin_wg_layout(NP, p.F, kMode, p.hp_max, p.stages).total;
+  DTB_CUDA_OK(cudaFuncSetAttribute(cin_wg_fwd_kernel<NP, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  // setmaxnreg only redistributes the registers the CTA got at launch: a smaller allocation would block the consumers
+  cudaFuncAttributes fa;
+  DTB_CUDA_OK(cudaFuncGetAttributes(&fa, cin_wg_fwd_kernel<NP, kMode>));
+  if (fa.numRegs * kFwdThreads < 2 * 128 * kFwdConsumerRegs + 128 * kFwdProducerRegs) {
+    set_error("dtb_cin_fwd: the CIN forward kernel was built with too few registers for its warpgroup split");
+    return DTB_ERR_CUDA;
+  }
+  const int n_pairs = (p.n_tiles + 1) / 2;
+  const int grid = n_pairs < sm_count() ? n_pairs : sm_count();
+  cin_wg_fwd_kernel<NP, kMode><<<grid, kFwdThreads, smem, st>>>(p);
   DTB_LAUNCH_OK();
   return DTB_OK;
 }
@@ -906,6 +1039,8 @@ int cin_wg_fwd(const CinShape& s, const int32_t* idx, const float* table, const 
   p.idx = idx; p.table = table; p.row_offsets = row_offsets; p.wpack = ws; p.bias = bias; p.pooled = pooled;
   p.saved = reinterpret_cast<float*>(saved); p.status = status; p.wmax = wmax;
   p.B = B; p.D = s.D; p.F = s.F; p.n_layers = s.n_layers; p.act = act; p.P = s.P;
+  p.n_tiles = (int)(((int64_t)B * s.D + kWgRows - 1) / kWgRows);
+  p.hp_max = cin_wg_hp_max(s); p.stages = cin_wg_fwd_stages(np, s.F, mode, p.hp_max);
   if (mode == 2) DTB_CUDA_OK(cudaMemsetAsync(wmax, 0, sizeof(int) * kCinMaxLayers, st));
   size_t woff = 0, soff = (size_t)B * s.D * s.F;
   for (int k = 0; k < s.n_layers; ++k) {

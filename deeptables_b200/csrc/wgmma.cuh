@@ -21,6 +21,22 @@ __device__ __forceinline__ void fence_barrier_init() {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// count arrivals at once (a reader that stands in for an absent one), by the threads where pred holds.  The predicate
+// sits on the instruction, not on a branch: a branch between wgmma groups in flight makes ptxas serialize them.
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, uint32_t count, bool pred) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %2, 0;\n\t"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0], %1;\n\t"
+      "}" ::"r"(smem_u32(bar)),
+      "r"(count), "r"((uint32_t)pred)
+      : "memory");
+}
+// named barrier: the first `threads` threads to arrive at barrier `id` (1..15; 0 is __syncthreads) wait for each other
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");

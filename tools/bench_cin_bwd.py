@@ -1,13 +1,16 @@
-"""Kernel times of the fused CIN backward at the headline shape (26 fields, D = 16, CIN 128x128x128, 65 536 rows):
-cin_wg_dgrad_kernel and each of the three cin_wg_wgrad_kernel launches, read from torch.profiler over repeated
-dtb_cin_bwd_phase calls with L2 flushed before each backward, as bench.py does.
+"""Kernel times of the fused CIN forward and backward at the headline shape (26 fields, D = 16, CIN 128x128x128,
+65 536 rows): cin_wg_fwd_kernel in training (activations saved) and in inference, cin_wg_dgrad_kernel and each of the
+three cin_wg_wgrad_kernel launches, read from torch.profiler over repeated dtb_cin_fwd and dtb_cin_bwd_phase calls
+with L2 flushed before each call, as bench.py does.
 
-    python tools/bench_cin_bwd.py [--batch 65536] [--iters 10]
+    python tools/bench_cin_bwd.py [--batch 65536] [--iters 10] [--precision 2]
 
-Prints ms per kernel and TFLOP/s per kernel: executed (what the tensor cores run: padded tiles, bf16x3 = 3 passes) and
-algorithmic (the FMAs of the math alone), both counted from the shape below, plus the card name and power limit.
-For the data gradient it also prints the bytes of weight chunks copied into shared memory and their rate; for each
-weight-gradient layer, the microseconds per 64-row block of its busiest CTA and the bytes bulk-copied per block.
+--precision is the forward's precision code (2 = bf16x3, 3 = one bf16 pass, 4 = one scaled fp16 pass); the backward
+runs bf16x3 for every code.  Prints ms per kernel and TFLOP/s per kernel: executed (what the tensor cores run: padded
+tiles, bf16x3 = 3 passes) and algorithmic (the FMAs of the math alone), both counted from the shape below, plus the
+card name and power limit.  For the forward and the data gradient it also prints the bytes of weight chunks copied
+into shared memory and their rate; for each weight-gradient layer, the microseconds per 64-row block of its busiest
+CTA and the bytes bulk-copied per block.
 """
 import argparse
 import ctypes
@@ -31,6 +34,17 @@ def _shape(b):
     while npj < max((h + 15) // 16 * 16 for h in H):
         npj *= 2
     return bd, n_blocks, H, npj
+
+
+def fwd_chunks(b, precision):
+    """Bytes of weight chunks cin_wg_fwd_kernel copies per call: one chunk per layer and x0 field (NP x Hp_k; bf16 hi +
+    lo for bf16x3, one 2-byte image otherwise) for each pair of 64-row tiles, which share every copy."""
+    bd, n_blocks, H, _ = _shape(b)
+    np_ = 16
+    while np_ < max(SIZES):
+        np_ *= 2
+    per_pair = sum(F * np_ * ((h + 15) // 16 * 16) * 2 * (2 if precision == 2 else 1) for h in H)
+    return per_pair * ((n_blocks + 1) // 2)
 
 
 def dgrad_chunks(b):
@@ -110,6 +124,8 @@ def flop_counts(b):
     while np_ < max(SIZES):
         np_ *= 2
     out = {}
+    fwd = (n_blocks * 64 * F * sum(np_ * ((h + 15) // 16 * 16) for h in H), bd * F * sum(h * s for h, s in zip(H, SIZES)))
+    out['cin_wg_fwd_kernel training'] = out['cin_wg_fwd_kernel inference'] = fwd
     nch, _, _ = dgrad_chunks(b)
     exe = sum(n_blocks * 64 * c * npj * ((s + 15) // 16 * 16) * 3 for c, s in zip(nch, SIZES))
     out['cin_wg_dgrad_kernel'] = (exe, sum(bd * F * h * s for h, s in zip(H, SIZES)))
@@ -138,6 +154,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--batch', type=int, default=65536)
     ap.add_argument('--iters', type=int, default=10)
+    ap.add_argument('--precision', type=int, default=2, choices=(2, 3, 4))
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -167,9 +184,28 @@ def main():
     gt = torch.zeros_like(table)
     dw = torch.zeros_like(w)
     P = lambda t: ctypes.c_void_p(t.data_ptr())
-    N.check(N.lib.dtb_cin_fwd(P(idx), P(table), P(offs), P(w), None, P(pooled), P(saved), P(ws), ws_bytes, b, F, D,
-                              sizes_c, n, 0, 1, 2, None, N.stream_ptr()), 'cin_fwd')
     flush = torch.zeros(512 << 20, dtype=torch.uint8, device=dev)
+
+    def fwd(sv, precision):
+        N.check(N.lib.dtb_cin_fwd(P(idx), P(table), P(offs), P(w), None, P(pooled), sv, P(ws), ws_bytes, b, F, D,
+                                  sizes_c, n, 0, 1, precision, None, N.stream_ptr()), 'cin_fwd')
+
+    for _ in range(3):
+        fwd(P(saved), args.precision)
+        fwd(None, args.precision)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(args.iters):
+            for sv in (P(saved), None):
+                flush.sum()
+                fwd(sv, args.precision)
+        torch.cuda.synchronize()
+    fwd_kern = sorted((e for e in prof.events() if 'cin_wg_fwd_kernel' in e.name), key=lambda e: e.time_range.start)
+    times = {}
+    for j, e in enumerate(fwd_kern):      # training and inference calls alternate
+        times.setdefault('cin_wg_fwd_kernel ' + ('training' if j % 2 == 0 else 'inference'), []).append(
+            e.time_range.elapsed_us() * 1e-3)
+    fwd(P(saved), 2)      # the backward reads the activations of a bf16x3 forward
 
     def bwd():
         for phase in (1, 2):
@@ -187,7 +223,6 @@ def main():
         torch.cuda.synchronize()
     kern = sorted((e for e in prof.events() if 'cin_wg_' in e.name),
                   key=lambda e: e.time_range.start)
-    times = {}
     wg_seen = 0
     for e in kern:
         if 'cin_wg_dgrad_kernel' in e.name:
@@ -200,7 +235,8 @@ def main():
         times.setdefault(key, []).append(e.time_range.elapsed_us() * 1e-3)
     flops = flop_counts(b)
     plans = wgrad_plan(b, torch.cuda.get_device_properties(0).multi_processor_count)
-    res = {'gpu': gpu_info(), 'batch': b, 'gemm_rows': b * D, 'iters': args.iters, 'kernels': {}}
+    res = {'gpu': gpu_info(), 'batch': b, 'gemm_rows': b * D, 'iters': args.iters, 'fwd_precision': args.precision,
+           'kernels': {}}
     wg_total = 0.0
     for key, (exe, alg) in flops.items():
         ts = sorted(times.get(key, []))
@@ -214,12 +250,17 @@ def main():
             res['kernels'].setdefault(key, {}).update(
                 us_per_block_per_cta=round(ms * 1e3 / pl['critical_blocks'], 3), bytes_per_block=pl['bytes_per_block'],
                 ctas=pl['ctas'], h_copy='tensor' if pl['htensor'] else ('rows' if pl['hpitch'] else 'none'))
+        if key.startswith('cin_wg_fwd') and args.precision == 2:
+            exe *= 3      # hi*hi, lo*hi, hi*lo
         res['kernels'].setdefault(key, {}).update(ms=round(ms, 4), executed_tflops=round(2 * exe / ms * 1e-9, 1),
                                                   algorithmic_tflops=round(2 * alg / ms * 1e-9, 1))
         if key == 'cin_wg_dgrad_kernel':
             # weight chunks bulk-copied from L2 into shared memory, one copy per tile and chunk
             _, tile_bytes, n_tiles = dgrad_chunks(b)
             gb = tile_bytes * n_tiles * 1e-9
+            res['kernels'][key].update(weight_chunk_gb=round(gb, 2), weight_chunk_gbps=round(gb / ms * 1e3, 1))
+        if key.startswith('cin_wg_fwd'):
+            gb = fwd_chunks(b, args.precision) * 1e-9
             res['kernels'][key].update(weight_chunk_gb=round(gb, 2), weight_chunk_gbps=round(gb / ms * 1e3, 1))
     res['wgrad_ms_total'] = round(wg_total, 4)
     print(json.dumps(res, indent=1))
