@@ -87,7 +87,6 @@ _SIGNATURES = {
                                   c_int, c_int, c_int, c_int, P]),
     'dtb_cin_tc_supported': (c_int, [c_int, c_int, _IP, c_int, c_int]),
     'dtb_cin_resolved_precision': (c_int, [c_int, c_int, _IP, c_int, c_int, c_int]),
-    'dtb_cin_tc_set_variant': (c_int, [c_int]),
     'dtb_tc_selftest': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cross_fwd': (c_int, [P, P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cross_bwd_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),

@@ -11,9 +11,6 @@ static bool is_fused_tc(int precision) {
   return precision == DTB_CIN_TC_BF16X3 || precision == DTB_CIN_TC_BF16X1 || precision == DTB_CIN_TC_F16X1;
 }
 
-// test hook (bit 16 of dtb_cin_tc_set_variant): the any-shape backward after a fused forward
-static int g_bwd_fp32 = 0;
-
 // auto: the fp32-grade bf16x3 fused forward where the shape fits it, else the any-shape formulation
 static int resolve_precision(const CinShape& s, int precision) {
   if (precision != DTB_CIN_AUTO) return precision;
@@ -98,13 +95,15 @@ static int cin_bwd_impl(const int32_t* idx, const float* table, const int64_t* r
   }
   if (B <= 0) return DTB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  if (is_fused_tc(resolve_precision(s, precision)) && !cin_wg_supported(s)) {
-    set_error("dtb_cin_bwd: tensor-core path requested but shape unsupported (F=%d D=%d)", F, D);
-    return DTB_ERR_UNSUPPORTED;
-  }
-  if (is_fused_tc(resolve_precision(s, precision)) && !g_bwd_fp32)
+  precision = resolve_precision(s, precision);
+  if (is_fused_tc(precision)) {
+    if (!cin_wg_supported(s)) {
+      set_error("dtb_cin_bwd: tensor-core path requested but shape unsupported (F=%d D=%d)", F, D);
+      return DTB_ERR_UNSUPPORTED;
+    }
     return cin_wg_bwd(s, idx, row_offsets, weights, d_pooled, saved, grad_table, d_weights, d_bias, workspace,
                       workspace_bytes, B, act, phase, st);
+  }
   return cin_fp32_bwd(s, idx, table, row_offsets, weights, d_pooled, saved, grad_table, d_weights, d_bias,
                       workspace, workspace_bytes, B, act, phase, st);
 }
@@ -124,11 +123,6 @@ int dtb_cin_bwd_phase(const int32_t* idx, const float* table, const int64_t* row
   DTB_CHECK_ARG(phase == 1 || phase == 2, "phase must be 1 (embedding gradient) or 2 (weight gradient)");
   return cin_bwd_impl(idx, table, row_offsets, weights, d_pooled, saved, grad_table, d_weights, d_bias, workspace,
                       workspace_bytes, B, F, D, layer_sizes_host, n_layers, direct, act, precision, phase, stream);
-}
-
-int dtb_cin_tc_set_variant(int variant) {
-  g_bwd_fp32 = (variant >> 16) & 1;
-  return DTB_OK;
 }
 
 }  // extern "C"

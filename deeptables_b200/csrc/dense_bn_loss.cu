@@ -133,18 +133,6 @@ static int ew_grid(int64_t total) {
 // ------------------------------------------------------------------------------------------
 // Dense epilogues and narrow (out_dim <= 8) logit layers
 // ------------------------------------------------------------------------------------------
-__global__ void bias_act_kernel(float* __restrict__ Y, const float* __restrict__ bias, int64_t total,
-                                int out_dim, int act) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    float v = Y[i];
-    if (bias) v += bias[i % out_dim];
-    if (act == DTB_ACT_RELU) v = fmaxf(v, 0.f);
-    else if (act == DTB_ACT_TANH) v = tanhf(v);
-    Y[i] = v;
-  }
-}
-
 __global__ void act_bwd_kernel(const float* __restrict__ Y, float* __restrict__ dY, int64_t total, int act) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {

@@ -275,7 +275,9 @@ int dtb_cin_bwd_phase(const int32_t* idx, const float* table, const int64_t* row
  *   1 = the any-shape materialising formulation (outer product in HBM chunks + the bf16x3 GEMMs of csrc/dense_tc.cu);
  *   2 = fused wgmma forward (csrc/cin_wgmma.cu: embedding dim 4/8/16/32, <= 64 fields, <= 64 hidden fields and <= 128
  *       feature maps per layer), bf16x3 split: fp32-grade; 3 = the same with one bf16 pass; 4 = one pass on fp16
- *       operands scaled by exact powers of two.  Codes 2-4 return DTB_ERR_UNSUPPORTED outside the fused shapes. */
+ *       operands scaled by exact powers of two.  Codes 2-4 return DTB_ERR_UNSUPPORTED outside the fused shapes.
+ * The backward takes its own precision: code 1 after a fused forward runs the any-shape backward on that forward's
+ * saved activations (both forwards save the same layout), which tests use as the reference for the fused backward. */
 #define DTB_CIN_AUTO 0
 #define DTB_CIN_FP32 1
 #define DTB_CIN_TC_BF16X3 2
@@ -284,12 +286,9 @@ int dtb_cin_bwd_phase(const int32_t* idx, const float* table, const int64_t* row
 int dtb_cin_tc_supported(int F, int D, const int* layer_sizes_host, int n_layers, int direct);
 /* which of the codes 1-4 a forward + backward with `precision` runs for this shape (0 = auto is resolved) */
 int dtb_cin_resolved_precision(int F, int D, const int* layer_sizes_host, int n_layers, int direct, int precision);
-/* Test hooks for the tensor-core path.  set_variant: bit 16 set runs the any-shape backward (exact-fp32 outer product)
- * instead of the fused one after a fused forward; every other bit is ignored (they chose between kernel variants of
- * the earlier sm_100a build).  selftest: C[128,N] = bf16(A[128,K]) @ bf16(Bmat[K,N]) on one warpgroup
+/* Test hook for the tensor-core path: C[128,N] = bf16(A[128,K]) @ bf16(Bmat[K,N]) on one warpgroup
  * (two m64 wgmma row blocks; N in {16, 32, 64, 128}, K <= 64 a multiple of 16), the A operand from registers
  * (a_operand_in_regs = 1) or from shared memory (0); workspace is not used and may be any non-NULL pointer. */
-int dtb_cin_tc_set_variant(int variant);
 int dtb_tc_selftest(const float* A, const float* Bmat, float* C, void* workspace, int N, int K,
                     int a_operand_in_regs, void* stream);
 

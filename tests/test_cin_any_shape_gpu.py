@@ -17,6 +17,7 @@ import numpy as np
 import pytest
 import torch
 
+import cin_ref
 from oracle import layers_ref as L
 
 pytestmark = pytest.mark.gpu
@@ -195,25 +196,6 @@ def cin64(x0, filt, bias, sizes, direct, act, d_pooled, masks=None, block_rows=N
                 T=[np.concatenate(v) for v in post], dx0=np.concatenate(dx0), dw=dw, db=db)
 
 
-def _cin_oracle(x, sizes, direct, filters, biases, act):
-    """oracle.layers_ref.cin with an identity head, one pooled column per call (as in tests/test_native_gpu.py)."""
-    params = dict(cross_layer_size=sizes, direct=direct, use_bias=biases is not None,
-                  activation='relu' if act else 'linear')
-    width = L.cin_pooled_width(x.shape[1], params)
-    w = {f'f_{k}': filters[k].unsqueeze(0) for k in range(len(sizes))}
-    if biases is not None:
-        for k in range(len(sizes)):
-            w[f'bias{k}'] = biases[k]
-    outs = []
-    for col in range(width):
-        kernel = torch.zeros(width, 1, dtype=x.dtype)
-        kernel[col, 0] = 1.0
-        w['exFM_out/kernel'] = kernel
-        w['exFM_out/bias'] = torch.zeros(1, dtype=x.dtype)
-        outs.append(L.cin(x, params, w))
-    return torch.cat(outs, dim=1)
-
-
 def make_weights(f, sizes, direct, use_bias, seed):
     """Filters scaled by 1 / (sqrt(K_k) * rms of the embeddings), which keeps every layer's activations near 1, so that
     the pooled columns of the last of 8 layers weigh as much in the check as those of the first."""
@@ -240,7 +222,7 @@ def test_float64_cin_matches_the_oracle(direct):
     x = torch.cat(L.embedding_lookup(t64, torch.tensor(idx)), dim=1)
     f64 = [torch.tensor(w, dtype=torch.float64, requires_grad=True) for w in filt]
     b64 = [torch.tensor(v, dtype=torch.float64, requires_grad=True) for v in bias]
-    want = _cin_oracle(x, sizes, direct, f64, b64, ACT_NONE)
+    want = cin_ref.cin_pooled_f64(x, sizes, direct, f64, b64, ACT_NONE)
     grads = torch.autograd.grad((want * torch.tensor(dp)).sum(), t64 + f64 + b64)
     pairs = [('pooled', ref['pooled'], want.detach().numpy()),
              ('table grad', scatter64(ref['dx0'], idx, tabs), torch.cat(grads[:f]).numpy())]

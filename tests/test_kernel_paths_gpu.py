@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 import torch
 
+import cin_ref
 from oracle import layers_ref as L
 
 pytestmark = pytest.mark.gpu
@@ -389,17 +390,6 @@ def conv_op(nat, b, h, w, cin, cout, kh, act):
     return make_op([k, bias], fwd, bwd, want, lambda w_: (1e-4, 1e-5))
 
 
-def _cin_oracle(x, sizes, direct, filters, biases, act):
-    params = dict(cross_layer_size=sizes, direct=direct, use_bias=biases is not None, activation='relu' if act else 'linear')
-    width = L.cin_pooled_width(x.shape[1], params)
-    w = {f'f_{k}': filters[k].unsqueeze(0) for k in range(len(sizes))}
-    for k in range(len(sizes) if biases is not None else 0):
-        w[f'bias{k}'] = biases[k]
-    w['exFM_out/kernel'] = torch.eye(width, dtype=x.dtype)      # identity head: the oracle returns the pooled features
-    w['exFM_out/bias'] = torch.zeros(width, dtype=x.dtype)
-    return L.cin(x, params, w)
-
-
 def cin_op(nat, f, d, sizes, b, precision):
     vocab = [9 + i for i in range(f)]
     tabs, flat, offs = make_table(vocab, d, seed=11)
@@ -431,9 +421,9 @@ def cin_op(nat, f, d, sizes, b, precision):
 
     def want():
         x = torch.cat(emb64(tabs, idx), dim=1)
-        return [_cin_oracle(x, sizes, False, [torch.tensor(w_, dtype=torch.float64) for w_ in filt],
-                            [torch.tensor(b_, dtype=torch.float64) for b_ in np.split(bias, np.cumsum(sizes)[:-1])],
-                            1).numpy()]
+        return [cin_ref.cin_pooled_f64(x, sizes, False, [torch.tensor(w_, dtype=torch.float64) for w_ in filt],
+                                       [torch.tensor(b_, dtype=torch.float64)
+                                        for b_ in np.split(bias, np.cumsum(sizes)[:-1])], 1).numpy()]
     tol = 1e-4 if precision == 1 else 1e-3                 # test_cin_fwd_bwd: fp32 path vs the bf16x3 tensor-core path
     return make_op([wcat, bias], fwd, bwd, want, lambda w_: (tol, tol * float(np.abs(w_[0]).max())))
 

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+import cin_ref
 from oracle import model_ref as M
 
 pytestmark = [pytest.mark.gpu]
@@ -85,25 +86,18 @@ def test_baseline_config_full_shape(case):
 # ---------------------------------------------------------------------------------------------------------------
 # DTB_CIN_TC_F16X1 (precision code 4): single tensor pass on power-of-two-scaled fp16 operands
 # ---------------------------------------------------------------------------------------------------------------
-# (F, sizes, direct, bias, act, B, D, kernel): 'v1' / 'v2' named the two fp16 forward kernels of the earlier sm_100a build,
-# selected by bit 18 of dtb_cin_tc_set_variant.  The sm_90a build has one (cin_wgmma.cu) and ignores that bit, so both ids
-# run it; the 'v1' cases are kept as extra shapes, and only 'v2' runs the backward comparison below.
-F16_CASES = [
-    (26, (128, 128, 128), False, False, 1, 37, 16, 'v2'),
-    (26, (128, 128, 128), False, False, 1, 37, 16, 'v1'),
-    (26, (32, 32, 16), False, True, 1, 64, 16, 'v2'),
-    (26, (32, 32, 16), False, True, 1, 64, 16, 'v1'),
-    (10, (64, 32), True, True, 1, 50, 16, 'v2'),
-    (10, (64, 32), True, True, 1, 50, 16, 'v1'),
-    (3, (32, 16), False, False, 0, 9, 16, 'v2'),
-    (3, (32, 16), False, False, 0, 9, 16, 'v1'),
-    (26, (128, 128), False, False, 1, 21, 32, 'v2'),
-    (40, (96, 64, 48), False, True, 1, 300, 16, 'v2'),      # F > 32: layer 0 is a 64-wide chunk too; ragged pooled split
+F16_CASES = [  # (F, sizes, direct, bias, act, B, D)
+    (26, (128, 128, 128), False, False, 1, 37, 16),
+    (26, (32, 32, 16), False, True, 1, 64, 16),
+    (10, (64, 32), True, True, 1, 50, 16),
+    (3, (32, 16), False, False, 0, 9, 16),
+    (26, (128, 128), False, False, 1, 21, 32),
+    (40, (96, 64, 48), False, True, 1, 300, 16),      # F > 32: layer 0 is a 64-wide chunk too; ragged pooled split
 ]
 
 
-@pytest.mark.parametrize('f,sizes,direct,use_bias,act,b,d,kernel', F16_CASES)
-def test_cin_fp16_single_pass_forward_is_inside_the_parity_bar(f, sizes, direct, use_bias, act, b, d, kernel):
+@pytest.mark.parametrize('f,sizes,direct,use_bias,act,b,d', F16_CASES)
+def test_cin_fp16_single_pass_forward_is_inside_the_parity_bar(f, sizes, direct, use_bias, act, b, d):
     """tools/cin_precision_study.py predicts max |err| of 2-6e-4 of the output scale for this scheme; the parity
     bar is rtol 1e-3 (+ atol 1e-4 of the scale).  Also checks the fused backward against the any-shape backward on
     the activations this forward saved."""
@@ -122,8 +116,7 @@ def test_cin_fp16_single_pass_forward_is_inside_the_parity_bar(f, sizes, direct,
     sizes_c, n = nat.int_array(sizes), len(sizes)
     if not nat.lib.dtb_cin_tc_supported(f, d, sizes_c, n, int(direct)):
         pytest.skip('shape not supported by the tensor-core kernels')
-    params = dict(cross_layer_size=sizes, direct=direct, use_bias=use_bias, activation='relu' if act else 'linear')
-    pw = L.cin_pooled_width(f, params)
+    pw = L.cin_pooled_width(f, dict(cross_layer_size=sizes, direct=direct))
     dev = lambda a: torch.tensor(a).cuda()                                   # noqa: E731
     d_idx, d_tab, d_offs = dev(idx), dev(table), dev(offs)
     d_w = dev(np.concatenate([x.reshape(-1) for x in filt]))
@@ -132,26 +125,14 @@ def test_cin_fp16_single_pass_forward_is_inside_the_parity_bar(f, sizes, direct,
     ws_bytes = nat.lib.dtb_cin_workspace_bytes(b, f, d, sizes_c, n, int(direct), 1)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device='cuda')
     saved = torch.empty(nat.lib.dtb_cin_saved_bytes(b, f, d, sizes_c, n, int(direct)), dtype=torch.uint8, device='cuda')
-    nat.lib.dtb_cin_tc_set_variant(1 | ((1 << 18) if kernel == 'v1' else 0))
-    try:
-        nat.check(nat.lib.dtb_cin_fwd(P(d_idx), P(d_tab), P(d_offs), P(d_w), P(d_b), P(pooled), P(saved), P(ws), ws_bytes,
-                                      b, f, d, sizes_c, n, int(direct), act, 4, None, None), 'cin_fwd fp16x1')
-        torch.cuda.synchronize()
-    finally:
-        nat.lib.dtb_cin_tc_set_variant(1)
-    # float64 reference of the pooled feature maps (the oracle's CIN up to the sum over D: identity output kernels)
+    nat.check(nat.lib.dtb_cin_fwd(P(d_idx), P(d_tab), P(d_offs), P(d_w), P(d_b), P(pooled), P(saved), P(ws), ws_bytes,
+                                  b, f, d, sizes_c, n, int(direct), act, 4, None, None), 'cin_fwd fp16x1')
+    torch.cuda.synchronize()
     t64 = torch.tensor(table, dtype=torch.float64)
     x = torch.stack([t64[offs[i] + torch.tensor(idx[:, i].astype(np.int64))] for i in range(f)], dim=1)
-    outs = []
-    for col in range(pw):
-        w = {f'f_{k}': torch.tensor(filt[k], dtype=torch.float64).unsqueeze(0) for k in range(n)}
-        if use_bias:
-            w.update({f'bias{k}': torch.tensor(bias[k], dtype=torch.float64) for k in range(n)})
-        kern = torch.zeros(pw, 1, dtype=torch.float64)
-        kern[col, 0] = 1.0
-        w['exFM_out/kernel'], w['exFM_out/bias'] = kern, torch.zeros(1, dtype=torch.float64)
-        outs.append(L.cin(x, params, w))
-    want = torch.cat(outs, dim=1).numpy()
+    want = cin_ref.cin_pooled_f64(x, sizes, direct, [torch.tensor(w_, dtype=torch.float64) for w_ in filt],
+                                  [torch.tensor(b_, dtype=torch.float64) for b_ in bias] if use_bias else None,
+                                  act).numpy()
     got = pooled.cpu().double().numpy()
     scale = np.abs(want).max()
     # one fp16 pass rounds each operand to 2^-11: the error of an output is ~3e-4 of the magnitude of its terms, NOT of
@@ -161,39 +142,34 @@ def test_cin_fp16_single_pass_forward_is_inside_the_parity_bar(f, sizes, direct,
     err = np.abs(got - want)
     assert err.max() / scale < 1e-3, f'max error {err.max() / scale:.2e} of the output scale'
     big = np.abs(want) > 1e-2 * scale
-    print(f'fp16x1 {kernel} F={f} sizes={sizes}: max err / scale {err.max() / scale:.2e}, '
+    print(f'fp16x1 F={f} sizes={sizes}: max err / scale {err.max() / scale:.2e}, '
           f'max rel err on entries > 1% of scale {(err[big] / np.abs(want[big])).max():.2e}')
     # elementwise: 1e-3 relative plus 1e-4 of the scale -- except for tiny reductions (F*H < 64 terms per output) where
     # the rounding errors of the few terms do not average out and the norm-wise bound above is all one fp16 pass gives
     if f * min(L.cin_field_nums(f, sizes, direct)) >= 64:
         bad = err > 1e-3 * np.abs(want) + 1e-4 * scale + 4e-4 * scale * (~big)
         assert not bad.any(), f'{int(bad.sum())} entries outside the bar, worst {err[bad].max() / scale:.2e} of the scale'
-    # backward: the fused wgmma backward of precision 4 against the exact-fp32 any-shape backward (bit 16) ON THE SAME
-    # saved activations (the fp16 forward's: a different forward flips relu-mask bits of near-zero outputs, which moves
-    # single gradient rows by percents and says nothing about the backward arithmetic)
+    # backward: the fused wgmma backward of precision 4 against the exact-fp32 any-shape backward (precision 1) ON THE
+    # SAME saved activations (the fp16 forward's: a different forward flips relu-mask bits of near-zero outputs, which
+    # moves single gradient rows by percents and says nothing about the backward arithmetic)
     d_dp = torch.randn(b, pw, device='cuda', generator=torch.Generator(device='cuda').manual_seed(5))
 
-    def backward(prec_b, flags):
-        nat.lib.dtb_cin_tc_set_variant(1 | flags)
-        try:
-            gt = torch.zeros(table.shape, device='cuda')
-            dw = torch.zeros_like(d_w)
-            db = torch.zeros(sum(sizes), device='cuda') if use_bias else None
-            nat.check(nat.lib.dtb_cin_bwd(P(d_idx), P(d_tab), P(d_offs), P(d_w), P(d_dp), P(saved), P(gt), P(dw), P(db), P(ws),
-                                          ws_bytes, b, f, d, sizes_c, n, int(direct), act, prec_b, None), 'cin_bwd')
-            torch.cuda.synchronize()
-            return gt, dw, db
-        finally:
-            nat.lib.dtb_cin_tc_set_variant(1)
+    def backward(prec_b):
+        gt = torch.zeros(table.shape, device='cuda')
+        dw = torch.zeros_like(d_w)
+        db = torch.zeros(sum(sizes), device='cuda') if use_bias else None
+        nat.check(nat.lib.dtb_cin_bwd(P(d_idx), P(d_tab), P(d_offs), P(d_w), P(d_dp), P(saved), P(gt), P(dw), P(db), P(ws),
+                                      ws_bytes, b, f, d, sizes_c, n, int(direct), act, prec_b, None), 'cin_bwd')
+        torch.cuda.synchronize()
+        return gt, dw, db
 
-    ref = backward(4, 1 << 16)  # the any-shape backward (fp32 outer product, bf16x3 GEMMs)
+    ref = backward(1)  # the any-shape backward (fp32 outer product, bf16x3 GEMMs)
     assert all(bool(torch.isfinite(t_).all()) for t_ in ref if t_ is not None) and float(ref[1].abs().max()) > 0
-    if kernel == 'v2':
-        got_g = backward(4, 0)
-        for name, r_, g_ in zip(('embedding', 'filter', 'bias'), ref, got_g):
-            if r_ is None:
-                continue
-            assert bool(torch.isfinite(g_).all())
-            rel = float((r_ - g_).abs().max() / r_.abs().max())
-            print(f'fused backward, {name} gradient vs the any-shape backward on the same activations: max err / max {rel:.2e}')
-            assert rel < 2e-3, f'{name} gradient off by {rel:.2e} of its maximum'
+    got_g = backward(4)
+    for name, r_, g_ in zip(('embedding', 'filter', 'bias'), ref, got_g):
+        if r_ is None:
+            continue
+        assert bool(torch.isfinite(g_).all())
+        rel = float((r_ - g_).abs().max() / r_.abs().max())
+        print(f'fused backward, {name} gradient vs the any-shape backward on the same activations: max err / max {rel:.2e}')
+        assert rel < 2e-3, f'{name} gradient off by {rel:.2e} of its maximum'

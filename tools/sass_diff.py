@@ -20,7 +20,8 @@ def kernels(path):
             name = m.group(1)
             d[name] = []
         elif name is not None:
-            d[name].append(re.sub(r'/\*[0-9a-f]{4}\*/', '', line).strip())     # drop instruction offsets
+            # drop instruction offsets, and the padding cuobjdump sizes to the longest instruction in the whole object
+            d[name].append(' '.join(re.sub(r'/\*[0-9a-f]{4}\*/', '', line).split()))
     return d
 
 
