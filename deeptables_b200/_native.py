@@ -75,7 +75,13 @@ _SIGNATURES = {
     'dtb_optim_rows_catchup_dev': (c_int, [P, P, P, P, P, P, P, P, _OPP, c_int, c_int, c_int, P]),
     'dtb_optim_rows_apply_dev': (c_int, [P, P, P, P, P, P, P, P, P, _OPP, c_int, c_int, c_int, P]),
     'dtb_optim_rows_flush_dev': (c_int, [P, P, P, P, P, P, _OPP, c_int64, c_int, P]),
-    'dtb_grad_rows_pack': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
+    'dtb_reg_grad': (c_int, [P, P, c_int64, c_float, c_float, P, c_double, P]),
+    'dtb_adam_dense_reg': (c_int, [P, P, P, P, c_int64, c_float, c_double, c_double, c_float, c_int, c_float, c_float,
+                                   P, c_double, P]),
+    'dtb_adam_dense_reg_dev': (c_int, [P, P, P, P, c_int64, P, P, c_double, c_double, c_float, c_int, c_float, c_float,
+                                       P, c_double, P]),
+    'dtb_optim_dense_reg': (c_int, [P, P, P, P, P, c_int64, _OPP, c_int, c_float, c_float, P, c_double, P]),
+    'dtb_grad_rows_pack':(c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),
     'dtb_cin_workspace_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int, c_int]),

@@ -16,6 +16,8 @@
 //     or near 0 keeps moving by them; then the whole gap is replayed.
 // Ownership of a row within one launch is claimed with atomicMax on last_step, so duplicate ids in a batch (and the
 // union of several ranks' ids) update the row exactly once.
+#include <initializer_list>
+
 #include "dtb_common.cuh"
 
 namespace dtb {
@@ -266,6 +268,181 @@ static int flush_impl(float* table, float* s0, float* s1, float* s2, int32_t* la
   return DTB_OK;
 }
 
+// ---- Keras weight regularizers (L1, L2, L1L2) ------------------------------------------------------------------------
+// Loss l1*sum|w| + l2*sum w^2 and gradient l1*sign(w) + 2*l2*w (sign(0) = 0, TensorFlow's gradient of abs).  The total
+// gradient is formed as g + (l1*sign(w) + (2*l2)*w) with every rounding pinned, in reg_grad_kernel* and in the fused
+// sweeps alike, so dtb_reg_grad followed by the plain sweep gives the fused sweep's bits.  The loss term is summed in
+// float64 from the weights before the step.
+struct RegArgs {
+  float l1, tl2;        // l1 and 2*l2 (exact in fp32)
+  double l2;
+  double* loss_acc;     // NULL: no loss term
+  double scale;
+};
+
+__device__ __forceinline__ float reg_total_grad(float g, float w, const RegArgs& r) {
+  const float s = w > 0.f ? 1.f : (w < 0.f ? -1.f : 0.f);
+  return __fadd_rn(g, __fadd_rn(__fmul_rn(r.l1, s), __fmul_rn(r.tl2, w)));
+}
+
+__device__ __forceinline__ void reg_sums(float w, double& a1, double& a2) {
+  const double d = (double)w;
+  a1 += fabs(d);
+  a2 = fma(d, d, a2);
+}
+
+// every thread of the block calls this once, after its loop
+__device__ __forceinline__ void reg_loss_flush(const RegArgs& r, double a1, double a2) {
+  __shared__ double part[32];
+  double v = warp_sum(r.scale * ((double)r.l1 * a1 + r.l2 * a2));
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) part[wid] = v;
+  __syncthreads();
+  if (wid == 0) {
+    v = warp_sum(lane < (int)(blockDim.x >> 5) ? part[lane] : 0.0);
+    if (lane == 0) atomicAdd(r.loss_acc, v);
+  }
+}
+
+// What a sweep does with (p, total g) at element i (scalar) or float4 index i; p and g are the values before the step.
+struct RegGradOnly {          // dtb_reg_grad: write the total gradient back (g may be NULL: loss only)
+  float* g;
+  __device__ void prepare() {}
+  __device__ void apply1(int64_t i, float, float gt) const { if (g) g[i] = gt; }
+  __device__ void apply4(int64_t i, float4, float4 gt) const { if (g) reinterpret_cast<float4*>(g)[i] = gt; }
+};
+
+struct AdamStep {
+  float *p, *m, *v, *g;
+  float alpha, omb1, omb2, eps;
+  const float* alpha_table;
+  const int32_t* step_dev;
+  int zero_grad;
+  __device__ void prepare() { if (step_dev) alpha = alpha_table[*step_dev + 1]; }
+  __device__ void apply1(int64_t i, float pi, float gt) const {
+    float mi = m[i], vi = v[i];
+    adam_update(pi, mi, vi, gt, alpha, omb1, omb2, eps);
+    p[i] = pi;
+    m[i] = mi;
+    v[i] = vi;
+    if (zero_grad) g[i] = 0.f;
+  }
+  __device__ void apply4(int64_t i, float4 p4, float4 g4) const {
+    float4 m4 = reinterpret_cast<float4*>(m)[i], v4 = reinterpret_cast<float4*>(v)[i];
+    adam_update(p4.x, m4.x, v4.x, g4.x, alpha, omb1, omb2, eps);
+    adam_update(p4.y, m4.y, v4.y, g4.y, alpha, omb1, omb2, eps);
+    adam_update(p4.z, m4.z, v4.z, g4.z, alpha, omb1, omb2, eps);
+    adam_update(p4.w, m4.w, v4.w, g4.w, alpha, omb1, omb2, eps);
+    reinterpret_cast<float4*>(p)[i] = p4;
+    reinterpret_cast<float4*>(m)[i] = m4;
+    reinterpret_cast<float4*>(v)[i] = v4;
+    if (zero_grad) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+};
+
+struct OptimStep {
+  float *p, *g, *s0, *s1, *s2;
+  OptimHP h;
+  int zero_grad;
+  __device__ void prepare() {}
+  __device__ void apply1(int64_t i, float pi, float gt) const {
+    float a = s0 ? s0[i] : 0.f, b = s1 ? s1[i] : 0.f, c = s2 ? s2[i] : 0.f;
+    optim_update(h, pi, a, b, c, gt);
+    p[i] = pi;
+    if (s0) s0[i] = a;
+    if (s1) s1[i] = b;
+    if (s2) s2[i] = c;
+    if (zero_grad) g[i] = 0.f;
+  }
+  __device__ void apply4(int64_t i, float4 p4, float4 g4) const {
+    const int64_t off = i * 4;
+    float4 a4 = load4_or_zero(s0, off), b4 = load4_or_zero(s1, off), c4 = load4_or_zero(s2, off);
+    optim_update4(h, p4, a4, b4, c4, g4);
+    *reinterpret_cast<float4*>(p + off) = p4;
+    store4_if(s0, off, a4);
+    store4_if(s1, off, b4);
+    store4_if(s2, off, c4);
+    if (zero_grad) *reinterpret_cast<float4*>(g + off) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+};
+
+template <class Op>
+__global__ void reg_sweep_kernel(const float* p, const float* g, int64_t n, RegArgs r, Op op) {
+  op.prepare();
+  double a1 = 0.0, a2 = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float w = p[i];
+    if (r.loss_acc) reg_sums(w, a1, a2);
+    op.apply1(i, w, reg_total_grad(g ? g[i] : 0.f, w, r));
+  }
+  if (r.loss_acc) reg_loss_flush(r, a1, a2);
+}
+
+template <class Op>
+__global__ void reg_sweep_vec4_kernel(const float* p, const float* g, int64_t n4, RegArgs r, Op op) {
+  op.prepare();
+  double a1 = 0.0, a2 = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    const float4 w = reinterpret_cast<const float4*>(p)[i];
+    if (r.loss_acc) {
+      reg_sums(w.x, a1, a2);
+      reg_sums(w.y, a1, a2);
+      reg_sums(w.z, a1, a2);
+      reg_sums(w.w, a1, a2);
+    }
+    const float4 g4 = g ? reinterpret_cast<const float4*>(g)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 gt = make_float4(reg_total_grad(g4.x, w.x, r), reg_total_grad(g4.y, w.y, r),
+                                  reg_total_grad(g4.z, w.z, r), reg_total_grad(g4.w, w.w, r));
+    op.apply4(i, w, gt);
+  }
+  if (r.loss_acc) reg_loss_flush(r, a1, a2);
+}
+
+static bool reg_factors_ok(float l1, float l2) {
+  return l1 >= 0.f && l2 >= 0.f && l1 <= 3.0e38f && l2 <= 1.0e38f;   // finite, non-negative, 2*l2 finite
+}
+
+static RegArgs to_reg(float l1, float l2, double* loss_acc, double loss_scale) {
+  return RegArgs{l1, 2.f * l2, (double)l2, loss_acc, loss_scale};
+}
+
+static bool all_aligned16(std::initializer_list<const void*> ptrs) {
+  uintptr_t bits = 0;
+  for (const void* q : ptrs) bits |= reinterpret_cast<uintptr_t>(q);
+  return (bits & 15) == 0;
+}
+
+// float4 sweep over the first n/4*4 elements when `aligned`, scalar kernel over the rest; `shift(op, k)` is op moved
+// k elements on
+template <class Op, class Shift>
+static int reg_sweep(const float* p, const float* g, int64_t n, bool aligned, const RegArgs& r, Op op, Shift shift,
+                     void* stream) {
+  if (n <= 0) return DTB_OK;
+  const int64_t n4 = aligned ? n / 4 : 0;
+  if (n4 > 0) {
+    reg_sweep_vec4_kernel<<<optim_grid(n4), 256, 0, (cudaStream_t)stream>>>(p, g, n4, r, op);
+    DTB_LAUNCH_OK();
+  }
+  const int64_t done = n4 * 4;
+  if (done < n) {
+    reg_sweep_kernel<<<optim_grid(n - done), 256, 0, (cudaStream_t)stream>>>(p + done, g ? g + done : nullptr, n - done,
+                                                                             r, shift(op, done));
+    DTB_LAUNCH_OK();
+  }
+  return DTB_OK;
+}
+
+static inline float* off_or_null(float* q, int64_t k) { return q ? q + k : nullptr; }
+
+static int adam_dense_reg_impl(float* p, float* m, float* v, float* g, int64_t n, float alpha, const float* alpha_table,
+                               const int32_t* step_dev, double beta1, double beta2, float eps, int zero_grad,
+                               const RegArgs& r, void* stream) {
+  // keras multiplies by the python double (1 - beta) rounded to fp32, as adam_dense_impl does
+  const AdamStep op{p, m, v, g, alpha, (float)(1.0 - beta1), (float)(1.0 - beta2), eps, alpha_table, step_dev, zero_grad};
+  return reg_sweep(p, g, n, all_aligned16({p, m, v, g}), r, op,
+                   [](AdamStep o, int64_t k) { o.p += k; o.m += k; o.v += k; o.g += k; return o; }, stream);
+}
+
 }  // namespace dtb
 
 using namespace dtb;
@@ -353,6 +530,52 @@ int dtb_optim_rows_flush_dev(float* table, float* s0, float* s1, float* s2, int3
   DTB_CHECK_HP(hp, s0, s1, s2);
   DTB_ROWS_SHAPE_OK(D);
   return flush_impl(table, s0, s1, s2, last_step, 0, step_dev, hp, n_rows, D, stream);
+}
+
+#define DTB_REG_FACTORS_OK(l1, l2) \
+  DTB_CHECK_ARG(reg_factors_ok(l1, l2), "regularization factors must be finite and non-negative")
+
+int dtb_reg_grad(const float* p, float* g, int64_t n, float l1, float l2, double* loss_acc, double loss_scale,
+                 void* stream) {
+  DTB_CHECK_ARG(p, "NULL argument");
+  DTB_REG_FACTORS_OK(l1, l2);
+  return reg_sweep(p, g, n, all_aligned16({p, g}), to_reg(l1, l2, loss_acc, loss_scale), RegGradOnly{g},
+                   [](RegGradOnly o, int64_t k) { o.g = off_or_null(o.g, k); return o; }, stream);
+}
+
+int dtb_adam_dense_reg(float* p, float* m, float* v, float* g, int64_t n, float alpha, double beta1, double beta2,
+                       float eps, int zero_grad, float l1, float l2, double* loss_acc, double loss_scale, void* stream) {
+  DTB_CHECK_ARG(p && m && v && g, "NULL argument");
+  DTB_REG_FACTORS_OK(l1, l2);
+  return adam_dense_reg_impl(p, m, v, g, n, alpha, nullptr, nullptr, beta1, beta2, eps, zero_grad,
+                             to_reg(l1, l2, loss_acc, loss_scale), stream);
+}
+
+int dtb_adam_dense_reg_dev(float* p, float* m, float* v, float* g, int64_t n, const float* alpha_table,
+                           const int32_t* step_dev, double beta1, double beta2, float eps, int zero_grad, float l1,
+                           float l2, double* loss_acc, double loss_scale, void* stream) {
+  DTB_CHECK_ARG(p && m && v && g && alpha_table && step_dev, "NULL argument");
+  DTB_REG_FACTORS_OK(l1, l2);
+  return adam_dense_reg_impl(p, m, v, g, n, 0.f, alpha_table, step_dev, beta1, beta2, eps, zero_grad,
+                             to_reg(l1, l2, loss_acc, loss_scale), stream);
+}
+
+int dtb_optim_dense_reg(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                        int zero_grad, float l1, float l2, double* loss_acc, double loss_scale, void* stream) {
+  DTB_CHECK_ARG(p && g, "NULL argument");
+  DTB_CHECK_HP(hp, s0, s1, s2);
+  DTB_REG_FACTORS_OK(l1, l2);
+  const OptimStep op{p, g, s0, s1, s2, to_hp(*hp), zero_grad};
+  return reg_sweep(p, g, n, all_aligned16({p, g, s0, s1, s2}), to_reg(l1, l2, loss_acc, loss_scale), op,
+                   [](OptimStep o, int64_t k) {
+                     o.p += k;
+                     o.g += k;
+                     o.s0 = off_or_null(o.s0, k);
+                     o.s1 = off_or_null(o.s1, k);
+                     o.s2 = off_or_null(o.s2, k);
+                     return o;
+                   },
+                   stream);
 }
 
 }  // extern "C"

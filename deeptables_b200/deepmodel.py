@@ -24,7 +24,7 @@ from typing import Union
 import numpy as np
 import torch
 
-from . import consts, deepnets, dp, engine as E, layers as L, optimizers as O
+from . import consts, deepnets, dp, engine as E, layers as L, optimizers as O, regularizers as R
 from ._native import ptr, check, stream_ptr
 from . import _native as N
 
@@ -37,6 +37,8 @@ class _Scope:
         self.generator = torch.Generator(device=self.device)
         self.generator.manual_seed(int(seed) if seed is not None else int.from_bytes(os.urandom(4), 'little'))
         self.params = OrderedDict()
+        self.regularizers = OrderedDict()  # parameter name -> regularizers.RegSpec (Keras add_weight(regularizer=))
+        self.reg_segments = []             # after freeze(): (offset, numel, l1, l2) of each regularized parameter
         self.stacked = {}                  # key of a param_stack() tensor -> the reference names of its slices
         self.buffers = OrderedDict()
         self.training = False
@@ -87,13 +89,16 @@ class _Scope:
         if self.capture is not None and name in self.capture:
             self.outputs[name] = out
 
-    def param(self, name, shape, init):
+    def param(self, name, shape, init, regularizer=None):
         p = self.params.get(name)
         if p is None:
             if self.frozen:
                 raise RuntimeError(f'parameter {name!r} requested after the model was built')
             p = L.init_tensor(shape, init, self.device, self.generator).requires_grad_(True)
             self.params[name] = p
+            spec = R.resolve(regularizer)
+            if spec is not None:
+                self.regularizers[name] = spec
         elif tuple(p.shape) != tuple(int(s) for s in shape):
             raise ValueError(f'parameter {name!r} has shape {tuple(p.shape)}, layer asked for {tuple(shape)}')
         return p
@@ -143,6 +148,7 @@ class _Scope:
             self.flat_slots = [None if s is None else torch.full((total,), s, dtype=torch.float32, device=self.device)
                                for s in slot_inits]
         off = 0
+        self.reg_segments = []
         for n, sz in zip(names, sizes):
             old = self.params[n]
             view = self.flat_p[off:off + sz].view(old.shape)
@@ -150,6 +156,8 @@ class _Scope:
             p = view.detach().requires_grad_(True)
             p.grad = self.flat_g[off:off + sz].view(old.shape)
             self.params[n] = p
+            if n in self.regularizers:
+                self.reg_segments.append((off, sz, self.regularizers[n].l1, self.regularizers[n].l2))
             off += sz
         self.frozen = True
 
@@ -262,6 +270,7 @@ class DeepModel:
         self._step_dev = None              # optimiser step counter in device memory (CUDA-graph replay of the train step)
         self._opt = None                   # optimizers.OptimizerSpec resolved from ModelConfig.optimizer
         self._opt_native = None            # its dtb_optim_params (SGD / RMSprop / Adagrad)
+        self._emb_reg = None               # regularizers.RegSpec of ModelConfig.embeddings_regularizer
         self._graphs = {}
         self._graph_failed = False
         if model_file is not None:
@@ -286,8 +295,8 @@ class DeepModel:
             self._focal = (cfg.loss.gamma, cfg.loss.alpha)
         elif cfg.loss != 'auto':
             raise NotImplementedError("loss must be 'auto' or one of layers.BinaryFocalLoss / CategoricalFocalLoss")
-        if cfg.embeddings_regularizer is not None or cfg.embeddings_activity_regularizer is not None:
-            raise NotImplementedError('embedding regularizers are outside the hot path')
+        R.reject_activity(cfg.embeddings_activity_regularizer, 'embeddings_activity_regularizer')
+        self._emb_reg = R.resolve(cfg.embeddings_regularizer, 'embeddings_regularizer')
         if self.task not in consts.ALL_TASKS:
             raise ValueError(f'Unknown task type:{self.task}')
         if len(set(self.emb_dims)) > 1:
@@ -301,6 +310,8 @@ class DeepModel:
                                           self.device, cfg.embeddings_initializer, self._scope.generator,
                                           field_dims=self.emb_dims)
             self.table.slot_inits = slot_inits
+            # a regularized table takes a non-zero gradient in every row every step: no exact-lazy row form
+            self.table.lazy_active = self.table.lazy_adam and self._emb_reg is None
         self.model_desc = ModelDesc()
         if self.n_fields:
             self.model_desc.add_input('all_categorical_vars', self.n_fields)
@@ -308,6 +319,8 @@ class DeepModel:
                                            list(self.emb_dims), cfg.embedding_dropout)
             if self.table.ragged:
                 self.model_desc.set_embedding_storage(self.table.dim, self.table.padding_share())
+            if self._emb_reg is not None:
+                self.model_desc.embeddings += f'\nregularizer: {self._emb_reg}'
         for c in self.continuous_columns:
             self.model_desc.add_input(c.name, c.input_dim)
         self.model_desc.set_dense(cfg.dense_dropout, False)
@@ -325,6 +338,7 @@ class DeepModel:
         with torch.no_grad():
             self._forward(cat, cont, training=False, describe=True)
         self._scope.freeze(slot_inits)
+        self.model_desc.regularizers = [f'{k}: {v}' for k, v in self._scope.regularizers.items()]
         dp.broadcast_parameters([self._scope.flat_p, self.table.weight if self.table is not None else None])
         self._loss_acc = torch.zeros(1, dtype=torch.float64, device=self.device)
         self.model = KerasLikeModel(self)
@@ -449,6 +463,7 @@ class DeepModel:
         want_lazy = bool(t.lazy_adam and n_refs * 6 <= t.total_rows)
         if getattr(self, '_table_mode_override', None) is not None:       # test hook
             want_lazy = bool(t.lazy_adam and self._table_mode_override == 'lazy')
+        want_lazy = want_lazy and self._emb_reg is None
         if want_lazy == t.lazy_active:
             return
         if t.lazy_active:                       # lazy -> dense: bring every row up to date first
@@ -522,9 +537,11 @@ class DeepModel:
         union_cat = cat
         if self._dist:
             union_cat = self._exchange_gradients(cat)
+        rows = y.shape[0]
+        self._reg_terms(scope.flat_g, self._loss_acc, rows)    # after the exchange: counted once, on every replica
         o = self._opt
         if o.kind != 'adam':
-            self._optim_step(union_cat, step, dev_step)
+            self._optim_step(union_cat, step, dev_step, rows)
             if dev_step:
                 check(N.lib.dtb_step_increment(ptr(self._step_dev), stream_ptr()), 'step_increment')
             return prob
@@ -538,6 +555,12 @@ class DeepModel:
                                                         ptr(t.grad), ptr(t.last_step), ptr(self._alpha), ptr(self._step_dev),
                                                         o.beta_1, o.beta_2, o.epsilon, union_cat.shape[0], t.n_fields,
                                                         t.dim, stream_ptr()), 'adam_rows_apply_dev')
+                elif self._emb_reg is not None:
+                    r = self._emb_reg
+                    check(N.lib.dtb_adam_dense_reg_dev(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(),
+                                                       ptr(self._alpha), ptr(self._step_dev), o.beta_1, o.beta_2,
+                                                       o.epsilon, 1, r.l1, r.l2, ptr(self._loss_acc), float(rows),
+                                                       stream_ptr()), 'adam_dense_reg_dev(table)')
                 else:
                     check(N.lib.dtb_adam_dense_dev(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(),
                                                    ptr(self._alpha), ptr(self._step_dev), o.beta_1, o.beta_2, o.epsilon, 1,
@@ -555,23 +578,33 @@ class DeepModel:
                                                 ptr(t.v), ptr(t.grad), ptr(t.last_step), ptr(a), step, o.beta_1,
                                                 o.beta_2, o.epsilon, union_cat.shape[0], t.n_fields, t.dim,
                                                 stream_ptr()), 'adam_rows_apply')
+            elif self._emb_reg is not None:
+                r = self._emb_reg
+                check(N.lib.dtb_adam_dense_reg(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(), alpha,
+                                               o.beta_1, o.beta_2, o.epsilon, 1, r.l1, r.l2, ptr(self._loss_acc),
+                                               float(rows), stream_ptr()), 'adam_dense_reg(table)')
             else:
                 check(N.lib.dtb_adam_dense(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(),
                                            alpha, o.beta_1, o.beta_2, o.epsilon, 1, stream_ptr()),
                       'adam_dense(table)')
         return prob
 
-    def _optim_step(self, union_cat, step, dev_step):
+    def _optim_step(self, union_cat, step, dev_step, rows):
         """SGD / RMSprop / Adagrad step `step`: the dense sweep over the flat parameters, then the table's row-wise
-        update (lazy) or dense sweep.  Only the row form needs the step number (to count skipped steps); its
-        CUDA-graph form reads it from device memory."""
+        update (lazy) or dense sweep (with the table's regularization fused in; `rows` scales its loss term).  Only
+        the row form needs the step number (to count skipped steps); its CUDA-graph form reads it from device
+        memory."""
         scope, t, hp = self._scope, self.table, self._opt_native
         check(N.lib.dtb_optim_dense(ptr(scope.flat_p), ptr(scope.flat_g), *[ptr(x) for x in scope.flat_slots],
                                     scope.flat_p.numel(), hp, 1, stream_ptr()), 'optim_dense')
         if t is None:
             return
         s = [ptr(x) for x in t.slots]
-        if not t.lazy_active:
+        if self._emb_reg is not None:
+            r = self._emb_reg
+            check(N.lib.dtb_optim_dense_reg(ptr(t.weight), ptr(t.grad), *s, t.weight.numel(), hp, 1, r.l1, r.l2,
+                                            ptr(self._loss_acc), float(rows), stream_ptr()), 'optim_dense_reg(table)')
+        elif not t.lazy_active:
             check(N.lib.dtb_optim_dense(ptr(t.weight), ptr(t.grad), *s, t.weight.numel(), hp, 1, stream_ptr()),
                   'optim_dense(table)')
         elif dev_step:
@@ -582,6 +615,22 @@ class DeepModel:
             check(N.lib.dtb_optim_rows_apply(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.grad),
                                              ptr(t.last_step), step, hp, union_cat.shape[0], t.n_fields, t.dim,
                                              stream_ptr()), 'optim_rows_apply')
+
+    def _reg_terms(self, flat_g, loss_acc, loss_scale):
+        """Regularized dense weights (Dense kernels): flat_g += their regularization gradient and loss_acc +=
+        loss_scale * their term, from the weights before the step.  flat_g None: the loss term only."""
+        scope = self._scope
+        for off, n, l1, l2 in scope.reg_segments:
+            check(N.lib.dtb_reg_grad(ptr(scope.flat_p[off:]), None if flat_g is None else ptr(flat_g[off:]), n, l1, l2,
+                                     ptr(loss_acc), float(loss_scale), stream_ptr()), 'reg_grad')
+
+    def _reg_loss(self, loss_acc, loss_scale):
+        """loss_acc += loss_scale * the regularization term of every regularized weight at the current weights."""
+        self._reg_terms(None, loss_acc, loss_scale)
+        if self._emb_reg is not None and self.table is not None:
+            r = self._emb_reg
+            check(N.lib.dtb_reg_grad(ptr(self.table.weight), None, self.table.weight.numel(), r.l1, r.l2, ptr(loss_acc),
+                                     float(loss_scale), stream_ptr()), 'reg_grad(table)')
 
     # ---- CUDA-graph replay of the train step ---------------------------------------------------------------------------
     def _has_dropout(self):
@@ -912,6 +961,7 @@ class DeepModel:
             probs.append(p)
             targets.append(by)
             seen += by.shape[0]
+        self._reg_loss(loss_acc, seen)          # Keras's compute_loss adds model.losses in evaluation too
         logs = {'loss': float(loss_acc.item()) / max(seen, 1)}
         pp, tt = torch.cat(probs), torch.cat(targets)
         for name, fn in metric_fns.items():
@@ -1231,6 +1281,7 @@ class ModelDesc:
         self.inputs, self.nets, self.nets_info = [], [], []
         self.embeddings = self.dense = self.concat_embed_dense = None
         self.stacking = self.output = self.loss = self.optimizer = None
+        self.regularizers = []             # 'weight name: regularizer' of the regularized Dense kernels
 
     def add_input(self, name, num_columns):
         self.inputs.append(f'{name}: ({num_columns})')
@@ -1266,6 +1317,8 @@ class ModelDesc:
                 ('concat_embed_dense', self.concat_embed_dense), ('nets', f'{self.nets}\n{self.nets_desc()}'),
                 ('stacking_op', self.stacking), ('output', self.output), ('loss', self.loss),
                 ('optimizer', self.optimizer_info())]
+        if self.regularizers:
+            rows.insert(5, ('regularizers', '\n'.join(self.regularizers)))
         body = f'\n{bar}\n'.join(f'{k}: {v}' for k, v in rows)
         return f'>>>>>>>>>>>>>>>>>>>>>> Model Desc <<<<<<<<<<<<<<<<<<<<<<< \n{bar}\n{body}\n{bar}\n'
 

@@ -312,15 +312,16 @@ def dnn(x, params, cellname='dnn'):
     hidden_units = params.get('hidden_units', ((128, 0, True), (64, 0, False)))
     activation = params.get('activation', 'relu')
     kernel_initializer = params.get('kernel_initializer', 'he_uniform')
-    if params.get('kernel_regularizer') is not None or params.get('activity_regularizer') is not None:
-        raise NotImplementedError('dnn regularizers are outside the hot path')
+    kernel_regularizer = params.get('kernel_regularizer')
+    activity_regularizer = params.get('activity_regularizer')
     if len(hidden_units) <= 0:
         raise ValueError(
             '[hidden_units] must be a list of tuple([units],[dropout_rate],[use_bn]) and at least one tuple.')
     for index, (units, dropout, batch_norm) in enumerate(hidden_units, start=1):
         x = Dense(units, use_bias=not batch_norm, name=f'{cellname}_dense_{index}',
                   activation=None if batch_norm else activation,
-                  kernel_initializer=kernel_initializer)(x)
+                  kernel_initializer=kernel_initializer, kernel_regularizer=kernel_regularizer,
+                  activity_regularizer=activity_regularizer)(x)
         if batch_norm:
             x = BatchNormalization(name=f'{cellname}_bn_{index}')(x)
             x = Activation(activation=activation, name=f'{cellname}_activation_{index}')(x)
@@ -334,11 +335,14 @@ def custom_dnn_D_A_D_B(x, params, cellname='dnn_D_A_D_B'):
     hidden_units = params.get('hidden_units', ((128, 0, True), (64, 0, False)))
     activation = params.get('activation', 'relu')
     kernel_initializer = params.get('kernel_initializer', 'he_uniform')
+    kernel_regularizer = params.get('kernel_regularizer')
+    activity_regularizer = params.get('activity_regularizer')
     if len(hidden_units) <= 0:
         raise ValueError(
             '[hidden_units] must be a list of tuple([units],[dropout_rate],[use_bn]) and at least one tuple.')
     for index, (units, dropout, batch_norm) in enumerate(hidden_units, start=1):
         x = Dense(units, activation=activation, kernel_initializer=kernel_initializer,
+                  kernel_regularizer=kernel_regularizer, activity_regularizer=activity_regularizer,
                   name=f'{cellname}_dense_{index}')(x)
         if dropout > 0:
             x = Dropout(dropout, name=f'{cellname}_dropout_{index}')(x)

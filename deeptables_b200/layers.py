@@ -15,7 +15,7 @@ import threading
 
 import torch
 
-from . import engine as E
+from . import engine as E, regularizers as R
 from .engine import FieldBlock, EmbeddingList
 
 _tls = threading.local()
@@ -91,6 +91,10 @@ class Layer:
     """Base: resolves the Keras-style unique layer name inside the active model scope."""
 
     def __init__(self, name=None, **kwargs):
+        regs = sorted(k for k, v in kwargs.items() if k.endswith('regularizer') and v is not None)
+        if regs:      # only Dense kernels and the embedding tables take regularizers, as in the reference
+            raise NotImplementedError(f'{type(self).__name__}({", ".join(regs)}): regularizers on this layer are not '
+                                      f'built natively')
         self._given_name = name
         self.name = name
 
@@ -118,15 +122,16 @@ class Dense(Layer):
         super().__init__(name)
         if activation not in E.ACT_CODES:
             raise NotImplementedError(f'activation {activation!r} (supported: relu, linear/None)')
-        if kernel_regularizer is not None or activity_regularizer is not None:
-            raise NotImplementedError('regularizers are outside the hot path')
+        R.reject_activity(activity_regularizer, 'Dense(activity_regularizer)')
+        self.kernel_regularizer = R.resolve(kernel_regularizer, 'Dense(kernel_regularizer)')
         self.units, self.activation, self.use_bias = int(units), activation, use_bias
         self.kernel_initializer = kernel_initializer
 
     def call(self, scope, x):
         x = _materialize(x)
         in_dim = x.shape[-1]
-        kernel = scope.param(f'{self.name}/kernel', (in_dim, self.units), self.kernel_initializer)
+        kernel = scope.param(f'{self.name}/kernel', (in_dim, self.units), self.kernel_initializer,
+                             regularizer=self.kernel_regularizer)
         bias = scope.param(f'{self.name}/bias', (self.units,), 'zeros') if self.use_bias else None
         return E.DenseFn.apply(x, kernel, bias, E.ACT_CODES[self.activation])
 

@@ -228,6 +228,24 @@ int dtb_optim_rows_apply_dev(const int32_t* idx, const int64_t* row_offsets, flo
 int dtb_optim_rows_flush_dev(float* table, float* s0, float* s1, float* s2, int32_t* last_step,
                              const int32_t* step_dev, const dtb_optim_params* hp, int64_t n_rows, int D, void* stream);
 
+/* ---- keras.regularizers L1 / L2 / L1L2 on a weight (add_weight(regularizer=)) ------------------ */
+/* Loss l1*sum|w| + l2*sum w^2, gradient l1*sign(w) + 2*l2*w with sign(0) = 0.  The total gradient is
+ * g + (l1*sign(w) + (2*l2)*w), rounded the same way by every entry point below, so dtb_reg_grad
+ * followed by dtb_adam_dense / dtb_optim_dense gives the bits of the fused *_reg sweep.
+ * dtb_reg_grad: g += gradient (g may be NULL: loss only).  All four add loss_scale * loss, summed in
+ * float64 from the weights before the step, into *loss_acc (may be NULL).  l1, l2 >= 0 and finite. */
+int dtb_reg_grad(const float* p, float* g, int64_t n, float l1, float l2, double* loss_acc, double loss_scale,
+                 void* stream);
+/* dtb_adam_dense / dtb_adam_dense_dev / dtb_optim_dense with the regularization gradient added to g
+ * in the same pass (no extra HBM traffic) */
+int dtb_adam_dense_reg(float* p, float* m, float* v, float* g, int64_t n, float alpha, double beta1, double beta2,
+                       float eps, int zero_grad, float l1, float l2, double* loss_acc, double loss_scale, void* stream);
+int dtb_adam_dense_reg_dev(float* p, float* m, float* v, float* g, int64_t n, const float* alpha_table,
+                           const int32_t* step_dev, double beta1, double beta2, float eps, int zero_grad, float l1,
+                           float l2, double* loss_acc, double loss_scale, void* stream);
+int dtb_optim_dense_reg(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                        int zero_grad, float l1, float l2, double* loss_acc, double loss_scale, void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
