@@ -81,6 +81,10 @@ _SIGNATURES = {
     'dtb_adam_dense_reg_dev': (c_int, [P, P, P, P, c_int64, P, P, c_double, c_double, c_float, c_int, c_float, c_float,
                                        P, c_double, P]),
     'dtb_optim_dense_reg': (c_int, [P, P, P, P, P, c_int64, _OPP, c_int, c_float, c_float, P, c_double, P]),
+    'dtb_optim_dense_lr': (c_int, [P, P, P, P, P, c_int64, _OPP, P, c_int, P, c_int, P]),
+    'dtb_optim_rows_apply_lr': (c_int, [P, P, P, P, P, P, P, P, P, c_int, P, _OPP, c_int, c_int, c_int, P]),
+    'dtb_optim_dense_reg_lr': (c_int, [P, P, P, P, P, c_int64, _OPP, P, c_int, P, c_int, c_float, c_float, P, c_double,
+                                       P]),
     'dtb_grad_rows_pack':(c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),

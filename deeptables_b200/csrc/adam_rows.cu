@@ -29,8 +29,15 @@ __device__ __forceinline__ void replay_zero_grad(float4& p, float4& m, float4& v
     adam_update(p.z, m.z, v.z, 0.f, a, omb1, omb2, eps);
     adam_update(p.w, m.w, v.w, 0.f, a, omb1, omb2, eps);
     // Long gaps (rare ids of a long-tailed column).  After ~1000 zero-gradient steps m reaches the fixed point of its
-    // decay (zero or the smallest denormals, |m| < 1e-44): from then on |m * alpha / (sqrt(v) + eps)| < 1e-40, which
-    // rounds away against any |p| > 1e-25 -- p and m no longer change and only the decay of v is left.
+    // decay (zero or the smallest denormals, |m| < 1e-44, so |m| <= 7 * 2^-149), and m stays there: its update with
+    // g = 0 reads m and omb1 alone.  Every later step then moves p by u = fl(fl(m * a) / d) with d = fl(sqrt(v)) + eps
+    // >= eps, and correctly rounded products and quotients are monotone, so |u| <= U = fl(fl(7 * 2^-149 * A) / eps)
+    // for every step whose alpha a is at most A.  |p| > 1e-25 puts p at or above the binade [2^-84, 2^-83), whose
+    // spacing is 2^-107: U < 2^-108 makes p - u round back to p.  p and m no longer change and only the decay of v is
+    // left.  The exit is valid as long as that holds for A = the largest alpha of the steps still to replay; the caller
+    // keeps the rows of a table whose alpha table breaks it on the dense sweep instead (DeepModel._select_table_optimizer).
+    // With a constant rate and Keras's defaults, 7 * 2^-149 * alpha rounds to 0, far inside the bound; a schedule that
+    // warms up, or a rate raised between epochs, can raise A, hence the check on the whole table.
     if (m.x == m0.x && m.y == m0.y && m.z == m0.z && m.w == m0.w && fabsf(m.x) < 1e-44f && fabsf(m.y) < 1e-44f &&
         fabsf(m.z) < 1e-44f && fabsf(m.w) < 1e-44f && fabsf(p.x) > 1e-25f && fabsf(p.y) > 1e-25f &&
         fabsf(p.z) > 1e-25f && fabsf(p.w) > 1e-25f) {

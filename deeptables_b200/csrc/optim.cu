@@ -9,11 +9,17 @@
 // replayed, in order and with the same device function (dtb_common.cuh), the next time the row is read or before the
 // table is exported.  The result is therefore bit-identical to the dense sweep by construction.
 //   * SGD without momentum and Adagrad: a zero-gradient step is the identity (p - 0*lr, acc + 0), nothing to replay.
-//   * SGD with momentum and RMSprop: a zero-gradient step decays the state and moves p by it.  The learning rate and
-//     every other hyperparameter are constants, so the step function does not depend on the step number: once one
-//     replayed step leaves p and every state word unchanged, all later ones do too and the replay stops there.  It
-//     does NOT stop when the state reaches zero: the smallest denormals are fixed points of x*0.9 and a parameter at
-//     or near 0 keeps moving by them; then the whole gap is replayed.
+//   * SGD with momentum and RMSprop: a zero-gradient step decays the state and moves p by it.  Every hyperparameter
+//     it uses is a constant, so the step function does not depend on the step number: once one replayed step leaves
+//     p and every state word unchanged, all later ones do too and the replay stops there.  It does NOT stop when the
+//     state reaches zero: the smallest denormals are fixed points of x*0.9 and a parameter at or near 0 keeps moving
+//     by them; then the whole gap is replayed.
+//
+// Learning-rate tables (the *_lr symbols): lr_table[s] is the rate of step s, read from device memory at step
+// *step_dev + 1 under CUDA-graph replay or at the host's `step` otherwise, so a schedule, or a rate a callback sets
+// between replays, reaches captured graphs.  The zero-gradient replay (catch-up and flush) never reads it: Keras's
+// SGD-momentum, RMSprop and Adagrad steps multiply the rate by g (dtb_common.cuh), so a g = 0 step does not depend on
+// the rate.  Only the steps that apply a gradient (dense sweep, row apply, regularized sweep) read the table.
 // Ownership of a row within one launch is claimed with atomicMax on last_step, so duplicate ids in a batch (and the
 // union of several ranks' ids) update the row exactly once.
 #include <initializer_list>
@@ -73,6 +79,16 @@ static const char* check_hp(const dtb_optim_params* h, const float* s0, const fl
     DTB_CHECK_ARG(_msg == nullptr, _msg);         \
   } while (0)
 
+// Where a launch takes its rate: hp.lr (table NULL), or table[*step_dev + 1] (graph form) / table[step] (host step).
+struct LrSource {
+  const float* table;
+  int step;
+  const int32_t* step_dev;
+  __device__ __forceinline__ void apply(OptimHP& h) const {
+    if (table) h.lr = table[step_dev ? *step_dev + 1 : step];
+  }
+};
+
 __device__ __forceinline__ void optim_update(const OptimHP& h, float& p, float& s0, float& s1, float& s2, float g) {
   if (h.kind == DTB_OPTIM_SGD)
     sgd_update(p, s0, g, h.lr, h.mu, h.flag);
@@ -117,7 +133,8 @@ __device__ __forceinline__ void optim_replay(const OptimHP& h, float4& p, float4
 // ---- dense sweep ---------------------------------------------------------------------------------------------------
 __global__ void optim_dense_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ s0,
                                    float* __restrict__ s1, float* __restrict__ s2, int64_t n, OptimHP h,
-                                   int zero_grad) {
+                                   int zero_grad, LrSource lr) {
+  lr.apply(h);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     float pi = p[i];
     float a = s0 ? s0[i] : 0.f, b = s1 ? s1[i] : 0.f, c = s2 ? s2[i] : 0.f;
@@ -132,7 +149,8 @@ __global__ void optim_dense_kernel(float* __restrict__ p, float* __restrict__ g,
 
 __global__ void optim_dense_vec4_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ s0,
                                         float* __restrict__ s1, float* __restrict__ s2, int64_t n4, OptimHP h,
-                                        int zero_grad) {
+                                        int zero_grad, LrSource lr) {
+  lr.apply(h);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t off = i * 4;
     float4 p4 = *reinterpret_cast<float4*>(p + off);
@@ -158,13 +176,16 @@ static int optim_grid(int64_t n) {
 // MODE 0: catch up to `step` (zero-gradient replay only)
 // MODE 1: apply step `step` with the accumulated gradient row, zero the gradient row
 // step_dev (CUDA-graph form): `step` is then an offset to *step_dev (0 = catch up, 1 = the next step)
+// lr_table (MODE 1 only): the rate of the applied step is lr_table[step], else h.lr
 template <int MODE>
 __global__ void optim_rows_kernel(const int32_t* __restrict__ idx, const int64_t* __restrict__ row_offsets,
                                   float* __restrict__ table, float* __restrict__ s0, float* __restrict__ s1,
                                   float* __restrict__ s2, float* __restrict__ grad, int32_t* __restrict__ last_step,
-                                  int step, OptimHP h, int B, int F, int D, const int32_t* __restrict__ step_dev) {
+                                  int step, OptimHP h, int B, int F, int D, const int32_t* __restrict__ step_dev,
+                                  const float* __restrict__ lr_table) {
   if (step_dev) step += *step_dev;
   if (step <= 0) return;
+  if (MODE == 1 && lr_table) h.lr = lr_table[step];
   const int Q = D >> 2;                      // lanes per row (power of two <= 32, checked by the host)
   const int64_t total = (int64_t)B * F * Q;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -241,17 +262,17 @@ static bool optim_rows_shape_ok(int D) {
 
 static int rows_impl(int mode, const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1,
                      float* s2, float* grad, int32_t* last_step, int step, const int32_t* step_dev,
-                     const dtb_optim_params* hp, int B, int F, int D, void* stream) {
+                     const dtb_optim_params* hp, int B, int F, int D, void* stream, const float* lr_table = nullptr) {
   if (B <= 0 || F <= 0) return DTB_OK;
   if (mode == 0 && zero_step_is_identity(*hp)) return DTB_OK;
   const int64_t total = (int64_t)B * F * (D / 4);
   const OptimHP h = to_hp(*hp);
   if (mode == 0)
     optim_rows_kernel<0><<<optim_grid(total), 256, 0, (cudaStream_t)stream>>>(
-        idx, row_offsets, table, s0, s1, s2, nullptr, last_step, step, h, B, F, D, step_dev);
+        idx, row_offsets, table, s0, s1, s2, nullptr, last_step, step, h, B, F, D, step_dev, nullptr);
   else
     optim_rows_kernel<1><<<optim_grid(total), 256, 0, (cudaStream_t)stream>>>(
-        idx, row_offsets, table, s0, s1, s2, grad, last_step, step, h, B, F, D, step_dev);
+        idx, row_offsets, table, s0, s1, s2, grad, last_step, step, h, B, F, D, step_dev, lr_table);
   DTB_LAUNCH_OK();
   return DTB_OK;
 }
@@ -344,7 +365,8 @@ struct OptimStep {
   float *p, *g, *s0, *s1, *s2;
   OptimHP h;
   int zero_grad;
-  __device__ void prepare() {}
+  LrSource lr;
+  __device__ void prepare() { lr.apply(h); }
   __device__ void apply1(int64_t i, float pi, float gt) const {
     float a = s0 ? s0[i] : 0.f, b = s1 ? s1[i] : 0.f, c = s2 ? s2[i] : 0.f;
     optim_update(h, pi, a, b, c, gt);
@@ -443,18 +465,10 @@ static int adam_dense_reg_impl(float* p, float* m, float* v, float* g, int64_t n
                    [](AdamStep o, int64_t k) { o.p += k; o.m += k; o.v += k; o.g += k; return o; }, stream);
 }
 
-}  // namespace dtb
-
-using namespace dtb;
-
 #define DTB_ROWS_SHAPE_OK(D) DTB_CHECK_ARG(optim_rows_shape_ok(D), "embedding dim must be 4*2^k (<=128) for the row-wise optimiser")
 
-extern "C" {
-
-int dtb_optim_dense(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
-                    int zero_grad, void* stream) {
-  DTB_CHECK_ARG(p && g, "NULL argument");
-  DTB_CHECK_HP(hp, s0, s1, s2);
+static int optim_dense_impl(float* p, float* g, float* s0, float* s1, float* s2, int64_t n,
+                            const dtb_optim_params* hp, int zero_grad, LrSource lr, void* stream) {
   if (n <= 0) return DTB_OK;
   const OptimHP h = to_hp(*hp);
   const bool aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) |
@@ -462,17 +476,69 @@ int dtb_optim_dense(float* p, float* g, float* s0, float* s1, float* s2, int64_t
                          reinterpret_cast<uintptr_t>(s2)) & 15) == 0;
   const int64_t n4 = aligned ? n / 4 : 0;
   if (n4 > 0) {
-    optim_dense_vec4_kernel<<<optim_grid(n4), 256, 0, (cudaStream_t)stream>>>(p, g, s0, s1, s2, n4, h, zero_grad);
+    optim_dense_vec4_kernel<<<optim_grid(n4), 256, 0, (cudaStream_t)stream>>>(p, g, s0, s1, s2, n4, h, zero_grad, lr);
     DTB_LAUNCH_OK();
   }
   const int64_t done = n4 * 4;
   if (done < n) {
     optim_dense_kernel<<<optim_grid(n - done), 256, 0, (cudaStream_t)stream>>>(
         p + done, g + done, s0 ? s0 + done : nullptr, s1 ? s1 + done : nullptr, s2 ? s2 + done : nullptr, n - done, h,
-        zero_grad);
+        zero_grad, lr);
     DTB_LAUNCH_OK();
   }
   return DTB_OK;
+}
+
+static int optim_dense_reg_impl(float* p, float* g, float* s0, float* s1, float* s2, int64_t n,
+                                const dtb_optim_params* hp, int zero_grad, LrSource lr, const RegArgs& r,
+                                void* stream) {
+  const OptimStep op{p, g, s0, s1, s2, to_hp(*hp), zero_grad, lr};
+  return reg_sweep(p, g, n, all_aligned16({p, g, s0, s1, s2}), r, op,
+                   [](OptimStep o, int64_t k) {
+                     o.p += k;
+                     o.g += k;
+                     o.s0 = off_or_null(o.s0, k);
+                     o.s1 = off_or_null(o.s1, k);
+                     o.s2 = off_or_null(o.s2, k);
+                     return o;
+                   },
+                   stream);
+}
+
+}  // namespace dtb
+
+using namespace dtb;
+
+extern "C" {
+
+int dtb_optim_dense(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                    int zero_grad, void* stream) {
+  DTB_CHECK_ARG(p && g, "NULL argument");
+  DTB_CHECK_HP(hp, s0, s1, s2);
+  return optim_dense_impl(p, g, s0, s1, s2, n, hp, zero_grad, LrSource{nullptr, 0, nullptr}, stream);
+}
+
+// the rate of step `step` (or *step_dev + 1 when step_dev is given) from lr_table; hp->lr is not read
+#define DTB_LR_SOURCE_OK(lr_table, step, step_dev) \
+  DTB_CHECK_ARG(lr_table && (step_dev || step >= 1), "lr_table is NULL or the host step is not 1-based")
+
+int dtb_optim_dense_lr(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                       const float* lr_table, int step, const int32_t* step_dev, int zero_grad, void* stream) {
+  DTB_CHECK_ARG(p && g, "NULL argument");
+  DTB_CHECK_HP(hp, s0, s1, s2);
+  DTB_LR_SOURCE_OK(lr_table, step, step_dev);
+  return optim_dense_impl(p, g, s0, s1, s2, n, hp, zero_grad, LrSource{lr_table, step, step_dev}, stream);
+}
+
+int dtb_optim_rows_apply_lr(const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1,
+                            float* s2, float* grad_table, int32_t* last_step, const float* lr_table, int step,
+                            const int32_t* step_dev, const dtb_optim_params* hp, int B, int F, int D, void* stream) {
+  DTB_CHECK_ARG(idx && row_offsets && table && grad_table && last_step, "NULL argument");
+  DTB_CHECK_HP(hp, s0, s1, s2);
+  DTB_ROWS_SHAPE_OK(D);
+  DTB_LR_SOURCE_OK(lr_table, step, step_dev);
+  return rows_impl(1, idx, row_offsets, table, s0, s1, s2, grad_table, last_step, step_dev ? 1 : step, step_dev, hp,
+                   B, F, D, stream, lr_table);
 }
 
 int dtb_optim_rows_catchup(const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1,
@@ -565,17 +631,19 @@ int dtb_optim_dense_reg(float* p, float* g, float* s0, float* s1, float* s2, int
   DTB_CHECK_ARG(p && g, "NULL argument");
   DTB_CHECK_HP(hp, s0, s1, s2);
   DTB_REG_FACTORS_OK(l1, l2);
-  const OptimStep op{p, g, s0, s1, s2, to_hp(*hp), zero_grad};
-  return reg_sweep(p, g, n, all_aligned16({p, g, s0, s1, s2}), to_reg(l1, l2, loss_acc, loss_scale), op,
-                   [](OptimStep o, int64_t k) {
-                     o.p += k;
-                     o.g += k;
-                     o.s0 = off_or_null(o.s0, k);
-                     o.s1 = off_or_null(o.s1, k);
-                     o.s2 = off_or_null(o.s2, k);
-                     return o;
-                   },
-                   stream);
+  return optim_dense_reg_impl(p, g, s0, s1, s2, n, hp, zero_grad, LrSource{nullptr, 0, nullptr},
+                              to_reg(l1, l2, loss_acc, loss_scale), stream);
+}
+
+int dtb_optim_dense_reg_lr(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                           const float* lr_table, int step, const int32_t* step_dev, int zero_grad, float l1, float l2,
+                           double* loss_acc, double loss_scale, void* stream) {
+  DTB_CHECK_ARG(p && g, "NULL argument");
+  DTB_CHECK_HP(hp, s0, s1, s2);
+  DTB_LR_SOURCE_OK(lr_table, step, step_dev);
+  DTB_REG_FACTORS_OK(l1, l2);
+  return optim_dense_reg_impl(p, g, s0, s1, s2, n, hp, zero_grad, LrSource{lr_table, step, step_dev},
+                              to_reg(l1, l2, loss_acc, loss_scale), stream);
 }
 
 }  // extern "C"

@@ -24,7 +24,7 @@ from typing import Union
 import numpy as np
 import torch
 
-from . import consts, deepnets, dp, engine as E, layers as L, optimizers as O, regularizers as R
+from . import consts, deepnets, dp, engine as E, layers as L, optimizers as O, regularizers as R, schedules as S
 from ._native import ptr, check, stream_ptr
 from . import _native as N
 
@@ -266,7 +266,7 @@ class DeepModel:
         self.table = None
         self._loss_acc = None
         self._focal = None                  # (gamma, alpha) when ModelConfig.loss is one of the focal losses
-        self._alpha = None
+        self._rates = None                 # _StepRates: the per-step learning rate (Adam: alpha) table in device memory
         self._step_dev = None              # optimiser step counter in device memory (CUDA-graph replay of the train step)
         self._opt = None                   # optimizers.OptimizerSpec resolved from ModelConfig.optimizer
         self._opt_native = None            # its dtb_optim_params (SGD / RMSprop / Adagrad)
@@ -283,6 +283,7 @@ class DeepModel:
         cfg = self.config
         self._opt = O.resolve(cfg.optimizer)
         self._opt_native = None if self._opt.kind == 'adam' else _native_optim_params(self._opt)
+        self._rates = _StepRates(self._opt, self.device)
         slot_inits = None if self._opt.kind == 'adam' else O.slot_inits(self._opt)
         self._focal = None
         if isinstance(cfg.loss, L.CategoricalFocalLoss):
@@ -447,12 +448,14 @@ class DeepModel:
     # one optimiser step / one scoring pass on device-resident batches
     # ------------------------------------------------------------------------------------------
     def _alpha_table(self, upto):
-        if self._alpha is None or self._alpha.numel() <= upto:
-            n = max(4096, 2 * (upto + 1))
-            o = self._opt
-            vals = [0.0] + [E.adam_alpha(s, o.learning_rate, o.beta_1, o.beta_2) for s in range(1, n)]
-            self._alpha = torch.tensor(vals, dtype=torch.float32, device=self.device)
-        return self._alpha
+        """The per-step table through step ``upto`` (Adam: alpha, the rate folded in; otherwise the rate)."""
+        self._rates.ensure(upto)
+        return self._rates.dev
+
+    @property
+    def optimizer(self):
+        """What Keras callbacks see as ``self.model.optimizer``: ``learning_rate`` (get / set) and ``iterations``."""
+        return _ModelOptimizer(self)
 
     def _select_table_optimizer(self, n_refs):
         """Row-wise exact-lazy Adam visits every touched row (the UNION over ranks in data parallel);
@@ -464,6 +467,10 @@ class DeepModel:
         if getattr(self, '_table_mode_override', None) is not None:       # test hook
             want_lazy = bool(t.lazy_adam and self._table_mode_override == 'lazy')
         want_lazy = want_lazy and self._emb_reg is None
+        # Adam's replay of long zero-gradient gaps stops early under a bound on the alphas it replays (adam_rows.cu):
+        # lazy for the coming step only while every alpha through it satisfies the bound.  A switch to dense flushes
+        # the steps done so far, all of which did.
+        want_lazy = want_lazy and self._rates.lazy_ok_through(self._step + 1)
         if want_lazy == t.lazy_active:
             return
         if t.lazy_active:                       # lazy -> dense: bring every row up to date first
@@ -492,7 +499,7 @@ class DeepModel:
             return
         if dev_step:          # CUDA-graph form: "steps done so far" is read from device memory
             check(N.lib.dtb_adam_rows_catchup_dev(ptr(cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m), ptr(t.v),
-                                                  ptr(t.last_step), ptr(self._alpha), ptr(self._step_dev), o.beta_1,
+                                                  ptr(t.last_step), ptr(self._rates.dev), ptr(self._step_dev), o.beta_1,
                                                   o.beta_2, o.epsilon, cat.shape[0], t.n_fields, t.dim, stream_ptr()),
                   'adam_rows_catchup_dev')
             return
@@ -510,6 +517,11 @@ class DeepModel:
         Single-GPU steps without dropout or sample weights are captured ONCE per batch shape in a CUDA graph and replayed
         (``DTB_CUDA_GRAPH=0`` disables it): a step is ~90 launches of kernels that take microseconds at small batch sizes
         (DeepFM at 8 192 rows), where the host's launch path -- not the GPU -- would set the pace."""
+        # the table covers this step before the table optimiser is chosen for it; a rate that overflowed is refused
+        # before anything runs
+        if self._rates.ensure(self._step + 1):
+            self._graphs.clear()                       # the table moved: captured pointers are stale
+        self._rates.check_step(self._step + 1)
         if self._graph_eligible(cat, cont, y, sample_weight):
             return self._train_step_graphed(cat, cont, y)
         prob = self._train_step_body(cat, cont, y, sample_weight, dev_step=False)
@@ -547,36 +559,35 @@ class DeepModel:
             return prob
         if dev_step:
             check(N.lib.dtb_adam_dense_dev(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
-                                           scope.flat_p.numel(), ptr(self._alpha), ptr(self._step_dev), o.beta_1,
+                                           scope.flat_p.numel(), ptr(self._rates.dev), ptr(self._step_dev), o.beta_1,
                                            o.beta_2, o.epsilon, 1, stream_ptr()), 'adam_dense_dev')
             if t is not None:
                 if t.lazy_active:
                     check(N.lib.dtb_adam_rows_apply_dev(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m), ptr(t.v),
-                                                        ptr(t.grad), ptr(t.last_step), ptr(self._alpha), ptr(self._step_dev),
+                                                        ptr(t.grad), ptr(t.last_step), ptr(self._rates.dev), ptr(self._step_dev),
                                                         o.beta_1, o.beta_2, o.epsilon, union_cat.shape[0], t.n_fields,
                                                         t.dim, stream_ptr()), 'adam_rows_apply_dev')
                 elif self._emb_reg is not None:
                     r = self._emb_reg
                     check(N.lib.dtb_adam_dense_reg_dev(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(),
-                                                       ptr(self._alpha), ptr(self._step_dev), o.beta_1, o.beta_2,
+                                                       ptr(self._rates.dev), ptr(self._step_dev), o.beta_1, o.beta_2,
                                                        o.epsilon, 1, r.l1, r.l2, ptr(self._loss_acc), float(rows),
                                                        stream_ptr()), 'adam_dense_reg_dev(table)')
                 else:
                     check(N.lib.dtb_adam_dense_dev(ptr(t.weight), ptr(t.m), ptr(t.v), ptr(t.grad), t.weight.numel(),
-                                                   ptr(self._alpha), ptr(self._step_dev), o.beta_1, o.beta_2, o.epsilon, 1,
+                                                   ptr(self._rates.dev), ptr(self._step_dev), o.beta_1, o.beta_2, o.epsilon, 1,
                                                    stream_ptr()), 'adam_dense_dev(table)')
             check(N.lib.dtb_step_increment(ptr(self._step_dev), stream_ptr()), 'step_increment')
             return prob
-        alpha = E.adam_alpha(step, o.learning_rate, o.beta_1, o.beta_2)
+        alpha = float(self._rates.host[step])          # the float32 the CUDA-graph form reads from the table
         check(N.lib.dtb_adam_dense(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
                                    scope.flat_p.numel(), alpha, o.beta_1, o.beta_2, o.epsilon, 1,
                                    stream_ptr()), 'adam_dense')
         if t is not None:
             if t.lazy_active:
-                a = self._alpha_table(step)
                 check(N.lib.dtb_adam_rows_apply(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m),
-                                                ptr(t.v), ptr(t.grad), ptr(t.last_step), ptr(a), step, o.beta_1,
-                                                o.beta_2, o.epsilon, union_cat.shape[0], t.n_fields, t.dim,
+                                                ptr(t.v), ptr(t.grad), ptr(t.last_step), ptr(self._rates.dev), step,
+                                                o.beta_1, o.beta_2, o.epsilon, union_cat.shape[0], t.n_fields, t.dim,
                                                 stream_ptr()), 'adam_rows_apply')
             elif self._emb_reg is not None:
                 r = self._emb_reg
@@ -591,30 +602,27 @@ class DeepModel:
 
     def _optim_step(self, union_cat, step, dev_step, rows):
         """SGD / RMSprop / Adagrad step `step`: the dense sweep over the flat parameters, then the table's row-wise
-        update (lazy) or dense sweep (with the table's regularization fused in; `rows` scales its loss term).  Only
-        the row form needs the step number (to count skipped steps); its CUDA-graph form reads it from device
-        memory."""
+        update (lazy) or dense sweep (with the table's regularization fused in; `rows` scales its loss term).  Each
+        reads the step's rate from the rate table: at `step`, or in the CUDA-graph form at the device counter + 1."""
         scope, t, hp = self._scope, self.table, self._opt_native
-        check(N.lib.dtb_optim_dense(ptr(scope.flat_p), ptr(scope.flat_g), *[ptr(x) for x in scope.flat_slots],
-                                    scope.flat_p.numel(), hp, 1, stream_ptr()), 'optim_dense')
+        lr = (ptr(self._rates.dev), 0, ptr(self._step_dev)) if dev_step else (ptr(self._rates.dev), step, None)
+        check(N.lib.dtb_optim_dense_lr(ptr(scope.flat_p), ptr(scope.flat_g), *[ptr(x) for x in scope.flat_slots],
+                                       scope.flat_p.numel(), hp, *lr, 1, stream_ptr()), 'optim_dense_lr')
         if t is None:
             return
         s = [ptr(x) for x in t.slots]
         if self._emb_reg is not None:
             r = self._emb_reg
-            check(N.lib.dtb_optim_dense_reg(ptr(t.weight), ptr(t.grad), *s, t.weight.numel(), hp, 1, r.l1, r.l2,
-                                            ptr(self._loss_acc), float(rows), stream_ptr()), 'optim_dense_reg(table)')
+            check(N.lib.dtb_optim_dense_reg_lr(ptr(t.weight), ptr(t.grad), *s, t.weight.numel(), hp, *lr, 1, r.l1,
+                                               r.l2, ptr(self._loss_acc), float(rows), stream_ptr()),
+                  'optim_dense_reg_lr(table)')
         elif not t.lazy_active:
-            check(N.lib.dtb_optim_dense(ptr(t.weight), ptr(t.grad), *s, t.weight.numel(), hp, 1, stream_ptr()),
-                  'optim_dense(table)')
-        elif dev_step:
-            check(N.lib.dtb_optim_rows_apply_dev(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.grad),
-                                                 ptr(t.last_step), ptr(self._step_dev), hp, union_cat.shape[0], t.n_fields,
-                                                 t.dim, stream_ptr()), 'optim_rows_apply_dev')
+            check(N.lib.dtb_optim_dense_lr(ptr(t.weight), ptr(t.grad), *s, t.weight.numel(), hp, *lr, 1, stream_ptr()),
+                  'optim_dense_lr(table)')
         else:
-            check(N.lib.dtb_optim_rows_apply(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.grad),
-                                             ptr(t.last_step), step, hp, union_cat.shape[0], t.n_fields, t.dim,
-                                             stream_ptr()), 'optim_rows_apply')
+            check(N.lib.dtb_optim_rows_apply_lr(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), *s, ptr(t.grad),
+                                                ptr(t.last_step), *lr, hp, union_cat.shape[0], t.n_fields, t.dim,
+                                                stream_ptr()), 'optim_rows_apply_lr')
 
     def _reg_terms(self, flat_g, loss_acc, loss_scale):
         """Regularized dense weights (Dense kernels): flat_g += their regularization gradient and loss_acc +=
@@ -656,9 +664,8 @@ class DeepModel:
                None if t is None else t.lazy_active)
         if self._step_dev is None:
             self._step_dev = torch.zeros(1, dtype=torch.int32, device=self.device)
-        if self._opt.kind == 'adam' and (self._alpha is None or self._alpha.numel() <= self._step + 2):
-            self._graphs.clear()                       # the alpha table moves when it grows: captured pointers are stale
-            self._alpha_table(self._step + 200000)
+        if self._rates.ensure(self._step + 2, reserve=200000):
+            self._graphs.clear()                       # the rate table moves when it grows: captured pointers are stale
         if t is not None:
             t.ensure_training_state()
             self._select_table_optimizer(cat.shape[0] * t.n_fields)
@@ -873,6 +880,7 @@ class DeepModel:
         for epoch in range(initial_epoch, epochs):
             for cb in callbacks:
                 _call(cb, 'on_epoch_begin', epoch, None)
+            self._agree_learning_rate()
             pdev = 'cpu' if on_host else self.device
             perm = torch.randperm(n, device=pdev) if shuffle else torch.arange(n, device=pdev)
             self._loss_acc.zero_()
@@ -921,14 +929,17 @@ class DeepModel:
                     torch.distributed.all_reduce(vt)
                     vlogs = dict(zip(keys, (vt / self.world_size).tolist()))
                 logs.update({f'val_{k}': v for k, v in vlogs.items()})
-            history.epoch.append(epoch)
-            for k, v in logs.items():
-                history.history.setdefault(k, []).append(v)
             if verbose:
                 msg = ' - '.join(f'{k}: {v:.4f}' for k, v in logs.items())
                 print(f'Epoch {epoch + 1}/{epochs} - {steps_per_epoch} steps - {msg}')
             for cb in callbacks:
                 _call(cb, 'on_epoch_end', epoch, logs)
+            self._agree_learning_rate()
+            # recorded after the callbacks, as Keras's History (the last callback) does: keys they add, such as
+            # ReduceLROnPlateau's 'learning_rate', are kept
+            history.epoch.append(epoch)
+            for k, v in logs.items():
+                history.history.setdefault(k, []).append(v)
             if self._dist:
                 # early stopping looks at per-rank validation metrics: stop everywhere as soon as one rank stops
                 flag = torch.tensor([1 if self.stop_training else 0], dtype=torch.int32, device=self.device)
@@ -940,6 +951,22 @@ class DeepModel:
             _call(cb, 'on_train_end', None)
         history.history = IgnoreCaseDict(history.history)
         return history
+
+    def _agree_learning_rate(self):
+        """Data parallel: every rank takes rank 0's learning rate before the next step.  A callback that set it on one
+        rank only (a decision on the per-rank training loss) would otherwise let the replicas drift apart."""
+        if not self._dist or self._rates is None:
+            return
+        ov = self._rates.override
+        t = torch.tensor([0.0 if ov is None else 1.0, 0.0 if ov is None else ov], dtype=torch.float64,
+                         device=self.device)
+        torch.distributed.broadcast(t, src=0)
+        flag, value = t.tolist()
+        if flag:
+            if value != ov:
+                self._rates.set(value, self._step)
+        elif ov is not None:
+            self._rates.clear_override(self._step)
 
     def _evaluate_tensors(self, cat, cont, y, batch_size, steps, metric_fns):
         n = y.shape[0]
@@ -1094,6 +1121,8 @@ class DeepModel:
         # (SGD / RMSprop / Adagrad: their state slots under __opt_slot{i}__ / __opt_table_slot{i}__); __optimizer__ names
         # the optimiser and its hyperparameters, under which alone the state resumes
         opt = {'__step__': np.array(self._step), '__optimizer__': np.array(self._opt.describe())}
+        if self._rates is not None and self._rates.override is not None:
+            opt['__learning_rate__'] = np.array(self._rates.override, dtype=np.float32)    # set by a callback
         if self._step > 0 and self._opt.kind != 'adam':
             for i, s in enumerate(self._scope.flat_slots):
                 if s is not None:
@@ -1158,6 +1187,8 @@ class DeepModel:
             self._step = step
         else:
             self._step = 0
+        if self._step > 0 and '__learning_rate__' in opt:
+            self._rates.set(float(opt['__learning_rate__']), self._step)
         if self._step_dev is not None:
             self._step_dev.fill_(self._step)
 
@@ -1194,6 +1225,157 @@ class _LazyFlat:
 class _NullDesc:
     def __getattr__(self, item):
         return lambda *a, **k: None
+
+
+class _StepRates:
+    """The per-step rate table in device memory.  ``dev[s]`` is what step ``s`` (1-based) reads: the learning rate for
+    SGD / RMSprop / Adagrad, Adam's alpha = rate * sqrt(1 - b2^s) / (1 - b1^s) with the rate folded in.  The rate of
+    step s is the schedule's at s - 1 completed steps, or the constant learning_rate; from the step after a callback
+    set it, the value set (float32), as with a Keras optimiser's learning-rate variable.  ``host`` mirrors ``dev``.
+
+    A set rewrites the entries of later steps in place, ordered on the current stream, so CUDA graphs that captured
+    ``dev`` read the new rates at their next replay.  Only growth reallocates ``dev`` (``ensure`` returns True).
+
+    The table runs ahead of training, and a schedule whose rate grows may overflow float32 at a step that never runs.
+    Entries are therefore stored as computed; ``check_step`` refuses a step whose entry is not finite and
+    non-negative when that step is about to run, and the table entries of later steps matter to nothing else."""
+
+    _TINY_M = np.float32(7 * 2.0 ** -149)       # largest |m| at the fixed point of Adam's zero-gradient decay
+    _HALF_SPACING = np.float32(2.0 ** -108)     # half the float32 spacing at |p| > 1e-25
+
+    def __init__(self, spec, device):
+        self.spec, self.device = spec, device
+        self.host = np.zeros(0, dtype=np.float32)
+        self.dev = None
+        self.override = None                    # float32 rate set by a callback, for every step after it was set
+        self._first_bad = 1 << 62               # first step whose entry is not finite and non-negative
+        self._first_break = 1 << 62             # first step whose Adam alpha breaks the lazy replay's bound
+
+    def _rates(self, s):
+        """float64 rates of steps s (int64 array, every s >= 1)."""
+        if self.override is not None:
+            return np.full(s.shape, self.override)
+        if self.spec.schedule is not None:
+            return S.rates(self.spec.schedule, s - 1, check=False)
+        return np.full(s.shape, self.spec.learning_rate)
+
+    def _values(self, s):
+        """float32 table entries of steps s (s = 0: unused, 0)."""
+        o = self.spec
+        one = np.maximum(s, 1)
+        r = self._rates(one)
+        if o.kind == 'adam':
+            # Python's float ** int (C pow) rather than np.power, whose vector form can differ in the last bit: a
+            # constant rate keeps the bits of engine.adam_alpha
+            steps = one.tolist()
+            b1 = np.fromiter(map(float(o.beta_1).__pow__, steps), dtype=np.float64, count=len(steps))
+            b2 = np.fromiter(map(float(o.beta_2).__pow__, steps), dtype=np.float64, count=len(steps))
+            r = r * np.sqrt(1.0 - b2) / (1.0 - b1)
+        with np.errstate(over='ignore', invalid='ignore'):
+            return np.where(s >= 1, r, 0.0).astype(np.float32)
+
+    def ensure(self, upto, reserve=0):
+        """Entries through step ``upto`` (and ``reserve`` more when it grows).  True when ``dev`` was reallocated."""
+        n_old = len(self.host)
+        if n_old > upto:
+            return False
+        n = max(4096, 2 * (upto + reserve + 1))
+        self.host = np.concatenate([self.host, self._values(np.arange(n_old, n, dtype=np.int64))])
+        self.dev = torch.from_numpy(self.host).to(self.device)
+        self._scan()
+        return True
+
+    def check_step(self, step):
+        """Raise ValueError naming learning_rate if step ``step`` would run at a rate (Adam: an alpha) that is not
+        finite and non-negative."""
+        if step >= self._first_bad:
+            raise ValueError(f'learning_rate: the rate of optimiser step {step} is {self.rate(step)!r} (table entry '
+                             f'{float(self.host[step])!r}); rates must be finite and non-negative')
+
+    def lazy_ok_through(self, step):
+        """Adam's exact-lazy replay may run steps 1..``step``: every alpha up to there satisfies its early-exit bound."""
+        return step < self._first_break
+
+    @property
+    def lazy_ok(self):
+        """lazy_ok_through every step the table holds."""
+        return self.lazy_ok_through(len(self.host) - 1)
+
+    def rate(self, step):
+        """The float32 learning rate of step ``step``."""
+        return float(np.float32(self._rates(np.array([max(step, 1)], dtype=np.int64))[0]))
+
+    def set(self, value, after):
+        """Every step after ``after`` takes float32(value)."""
+        v = float(np.float32(value))
+        if not np.isfinite(v) or v < 0:
+            raise ValueError(f'learning_rate must be finite and non-negative, got {value!r}')
+        self.override = v
+        self._rewrite(after)
+
+    def clear_override(self, after):
+        """Steps after ``after`` follow the schedule (or the constant rate) again."""
+        self.override = None
+        self._rewrite(after)
+
+    def _rewrite(self, after):
+        lo = after + 1
+        if lo < len(self.host):
+            vals = self._values(np.arange(lo, len(self.host), dtype=np.int64))
+            self.host[lo:] = vals
+            self.dev[lo:].copy_(torch.from_numpy(vals))
+        self._scan()
+
+    def _scan(self):
+        """First bad entry, and first entry that breaks Adam's replay bound.  The lazy replay stops a long
+        zero-gradient gap early where fl(fl(7 * 2^-149 * A) / eps) < 2^-108 for A = the largest alpha it replays
+        (adam_rows.cu), evaluated here in float32 like the kernels.  A replay of steps 1..s only ever uses their
+        alphas, so the table rows may go lazy for step s while every entry up to s satisfies the bound (a prefix);
+        entries of steps that have not run yet do not matter."""
+        v = self.host[1:]
+        bad = ~(np.isfinite(v) & (v >= 0))
+        self._first_bad = 1 + int(np.argmax(bad)) if bad.any() else 1 << 62
+        if self.spec.kind != 'adam':
+            return
+        with np.errstate(over='ignore', divide='ignore', invalid='ignore'):
+            u = (self._TINY_M * v) / np.float32(self.spec.epsilon)
+        brk = ~(u < self._HALF_SPACING)
+        self._first_break = 1 + int(np.argmax(brk)) if brk.any() else 1 << 62
+
+
+class _ModelOptimizer:
+    """``DeepModel.optimizer``: the part of a Keras optimiser that callbacks use."""
+
+    def __init__(self, model):
+        self._model = model
+
+    @property
+    def iterations(self):
+        """Optimiser steps completed."""
+        return self._model._step
+
+    @property
+    def learning_rate(self):
+        """The rate the next step will use (float32, as a Python float)."""
+        m = self._model
+        if m._rates is None:
+            m._build_model()
+        return m._rates.rate(m._step + 1)
+
+    @learning_rate.setter
+    def learning_rate(self, value):
+        m = self._model
+        if m._rates is None:
+            m._build_model()
+        if m._opt.schedule is not None:
+            raise TypeError('This optimizer was created with a `LearningRateSchedule` object as its `learning_rate` '
+                            'constructor argument, hence its learning rate is not settable.  If you need the learning '
+                            'rate to be settable, you should instantiate the optimizer with a float `learning_rate` '
+                            'argument.')
+        m._rates.set(float(value), m._step)
+
+    def __repr__(self):
+        return f'<{self._model._opt.keras_name} learning_rate={self.learning_rate} iterations={self.iterations}>'
 
 
 def _native_optim_params(spec):

@@ -6,14 +6,20 @@ below, or any object of one of those four class names with ``get_config()`` -- a
 included, as in the reference's own example.  ``resolve`` turns each of them into an ``OptimizerSpec``: a plain,
 hashable description that the engine runs and that checkpoints record.
 
+``learning_rate`` is a non-negative number or one of Keras 3's built-in schedules (``schedules.py``), in any form
+``schedules.resolve`` accepts.
+
 Every trainable weight, every embedding row included, takes a step every iteration (Keras's dense semantics; a row
-with no gradient steps with g = 0).  Learning-rate schedules, weight decay, clipping, EMA, loss scaling, gradient
-accumulation, AMSGrad and the other Keras optimisers are not built: ``resolve`` rejects them with
+with no gradient steps with g = 0).  Custom learning-rate schedules, weight decay, clipping, EMA, loss scaling,
+gradient accumulation, AMSGrad and the other Keras optimisers are not built: ``resolve`` rejects them with
 ``NotImplementedError`` naming the option.
 """
 import json
+import math
 import numbers
 from typing import NamedTuple, Optional
+
+from . import schedules as S
 
 # keyword -> default of keras.optimizers.Optimizer (Keras 3) that every optimiser class accepts
 _BASE_DEFAULTS = dict(weight_decay=None, clipnorm=None, clipvalue=None, global_clipnorm=None, use_ema=False,
@@ -35,6 +41,7 @@ class OptimizerSpec(NamedTuple):
     rho: Optional[float] = None                 # rmsprop
     centered: Optional[bool] = None             # rmsprop
     initial_accumulator_value: Optional[float] = None   # adagrad
+    schedule: Optional[tuple] = None            # schedules.resolve description; learning_rate is then its step-1 rate
 
     @property
     def keras_name(self):
@@ -43,7 +50,10 @@ class OptimizerSpec(NamedTuple):
 
     def describe(self):
         """Stable text form, stored in checkpoints: a saved optimiser state resumes only under the same description."""
-        return json.dumps(self._asdict(), sort_keys=True)
+        d = self._asdict()
+        if d['schedule'] is None:       # the text of an optimiser without a schedule is what it always was
+            del d['schedule']
+        return json.dumps(d, sort_keys=True)
 
 
 class _KerasOptimizer:
@@ -132,26 +142,36 @@ def resolve(optimizer):
         if not (value == default or (key == 'weight_decay' and value == 0)):
             raise NotImplementedError(f'{cls_name}({key}={value!r}) is not built natively: weight decay, clipping, '
                                       f'EMA, loss scaling and gradient accumulation are not supported')
-    lr = cfg['learning_rate']
-    if isinstance(lr, bool) or not isinstance(lr, numbers.Real):
-        raise NotImplementedError(f'{cls_name}(learning_rate={lr!r}): learning-rate schedules are not built natively; '
-                                  f'pass a number')
-    lr = float(lr)
+    lr, sched = _learning_rate(cls_name, cfg['learning_rate'])
     if cls_name == 'Adam':
         if cfg['amsgrad']:
             raise NotImplementedError('Adam(amsgrad=True) is not built natively')
         return OptimizerSpec('adam', lr, beta_1=float(cfg['beta_1']), beta_2=float(cfg['beta_2']),
-                             epsilon=float(cfg['epsilon']))
+                             epsilon=float(cfg['epsilon']), schedule=sched)
     if cls_name == 'SGD':
         momentum = float(cfg['momentum'])
         if not 0.0 <= momentum <= 1.0:
             raise ValueError(f'SGD momentum must be in [0, 1], got {momentum}')
-        return OptimizerSpec('sgd', lr, momentum=momentum, nesterov=bool(cfg['nesterov']))
+        return OptimizerSpec('sgd', lr, momentum=momentum, nesterov=bool(cfg['nesterov']), schedule=sched)
     if cls_name == 'RMSprop':
         return OptimizerSpec('rmsprop', lr, epsilon=float(cfg['epsilon']), momentum=float(cfg['momentum']),
-                             rho=float(cfg['rho']), centered=bool(cfg['centered']))
+                             rho=float(cfg['rho']), centered=bool(cfg['centered']), schedule=sched)
     return OptimizerSpec('adagrad', lr, epsilon=float(cfg['epsilon']),
-                         initial_accumulator_value=float(cfg['initial_accumulator_value']))
+                         initial_accumulator_value=float(cfg['initial_accumulator_value']), schedule=sched)
+
+
+def _learning_rate(cls_name, lr):
+    """learning_rate -> (rate of the first step, schedule description or None)."""
+    if isinstance(lr, bool) or not isinstance(lr, numbers.Real):
+        try:
+            sched = S.resolve(lr)
+        except NotImplementedError as exc:
+            raise NotImplementedError(f'{cls_name}(learning_rate=...): {exc}') from None
+        return float(S.rates(sched, [0])[0]), sched
+    lr = float(lr)
+    if not math.isfinite(lr) or lr < 0:
+        raise ValueError(f'{cls_name}(learning_rate={lr!r}): the learning rate must be finite and non-negative')
+    return lr, None
 
 
 def slot_inits(spec):

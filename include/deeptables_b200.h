@@ -156,7 +156,9 @@ int dtb_adam_dense(float* p, float* m, float* v, float* g, int64_t n, float alph
 /* Exact-lazy row-wise Adam for embedding tables (same arithmetic as dtb_adam_dense applied to
  * every row every step, but rows whose gradient is zero are caught up only when next touched).
  * last_step[row] = last optimiser step already applied to that row.  alpha_table[s] (device,
- * s = 1..) = alpha of step s.
+ * s = 1..) = alpha of step s (a learning-rate schedule is folded into it).  The replay of long
+ * zero-gradient gaps stops early under a bound that holds while
+ * fl(fl(7 * 2^-149 * max alpha) / eps) < 2^-108 (adam_rows.cu); the caller keeps tables past it dense.
  *   catchup: for every (b,f): apply the zero-gradient steps last_step+1 .. upto to that row once.
  *   apply  : for every (b,f): apply step `step` with the accumulated grad_table row once, zero
  *            the grad row, set last_step = step. */
@@ -186,7 +188,8 @@ int dtb_step_increment(int32_t* step_dev, void* stream);
 
 /* ---- keras SGD, RMSprop and Adagrad, dense semantics (optim.cu) ----------------------------------
  * Hyperparameters travel in a host-side struct read at call time (a captured graph keeps the values
- * of the call it captured; none of them changes during training).  State slots s0..s2 are [n] floats
+ * of the call it captured).  The learning rate may instead come from a device table (the *_lr forms
+ * below), which is how a schedule or a rate changed during training reaches a captured graph.  State slots s0..s2 are [n] floats
  * like p, NULL when the optimiser does not use them:
  *   SGD     s0 = momentum buffer (when momentum > 0)
  *   RMSprop s0 = velocity, s1 = average gradient (centered), s2 = momentum buffer (momentum > 0)
@@ -227,6 +230,16 @@ int dtb_optim_rows_apply_dev(const int32_t* idx, const int64_t* row_offsets, flo
                              const dtb_optim_params* hp, int B, int F, int D, void* stream);
 int dtb_optim_rows_flush_dev(float* table, float* s0, float* s1, float* s2, int32_t* last_step,
                              const int32_t* step_dev, const dtb_optim_params* hp, int64_t n_rows, int D, void* stream);
+/* Learning-rate table forms of the steps that apply a gradient: dtb_optim_dense, dtb_optim_rows_apply(_dev) and
+ * dtb_optim_dense_reg with the rate of step s read from lr_table[s] (device, s = 1..) instead of hp->lr.  The step
+ * is *step_dev + 1 when step_dev is not NULL (CUDA-graph replay), else the host's `step` (>= 1).  With a table
+ * that holds hp->lr at that step they give the bits of the constant-rate symbols.  The zero-gradient catch-up and
+ * flush need no table: a g = 0 step of SGD, RMSprop or Adagrad does not depend on the rate. */
+int dtb_optim_dense_lr(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                       const float* lr_table, int step, const int32_t* step_dev, int zero_grad, void* stream);
+int dtb_optim_rows_apply_lr(const int32_t* idx, const int64_t* row_offsets, float* table, float* s0, float* s1,
+                            float* s2, float* grad_table, int32_t* last_step, const float* lr_table, int step,
+                            const int32_t* step_dev, const dtb_optim_params* hp, int B, int F, int D, void* stream);
 
 /* ---- keras.regularizers L1 / L2 / L1L2 on a weight (add_weight(regularizer=)) ------------------ */
 /* Loss l1*sum|w| + l2*sum w^2, gradient l1*sign(w) + 2*l2*w with sign(0) = 0.  The total gradient is
@@ -245,6 +258,10 @@ int dtb_adam_dense_reg_dev(float* p, float* m, float* v, float* g, int64_t n, co
                            float l2, double* loss_acc, double loss_scale, void* stream);
 int dtb_optim_dense_reg(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
                         int zero_grad, float l1, float l2, double* loss_acc, double loss_scale, void* stream);
+/* dtb_optim_dense_reg with the rate from lr_table, as dtb_optim_dense_lr */
+int dtb_optim_dense_reg_lr(float* p, float* g, float* s0, float* s1, float* s2, int64_t n, const dtb_optim_params* hp,
+                           const float* lr_table, int step, const int32_t* step_dev, int zero_grad, float l1, float l2,
+                           double* loss_acc, double loss_scale, void* stream);
 
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
