@@ -56,6 +56,8 @@ _SIGNATURES = {
     'dtb_dense_fwd': (c_int, [P, P, P, P, P, c_size_t, c_int, c_int, c_int, c_int, P]),
     'dtb_dense_bwd': (c_int, [P, P, P, P, P, P, P, P, c_size_t, c_int, c_int, c_int, c_int, P]),
     'dtb_dropout': (c_int, [P, P, c_int64, c_float, c_ulonglong, P]),
+    'dtb_dropout_dev': (c_int, [P, P, c_int64, c_float, P, P]),
+    'dtb_seed_advance': (c_int, [P, c_int, P]),
     'dtb_loss_fwd_bwd': (c_int, [P, P, P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_focal_loss_fwd_bwd': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_float, c_float, P]),
     'dtb_adam_dense': (c_int, [P, P, P, P, c_int64, c_float, c_double, c_double, c_float, c_int, P]),
@@ -118,6 +120,10 @@ _SIGNATURES = {
     'dtb_maxpool_fields_bwd': (c_int, [P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_attention_core_fwd': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P]),
     'dtb_attention_core_bwd': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    'dtb_attention_core_dropout_fwd': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_float, c_ulonglong, P,
+                                               c_longlong, P]),
+    'dtb_attention_core_dropout_bwd': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
+                                               c_ulonglong, P, c_longlong, P]),
 }
 
 

@@ -360,17 +360,17 @@ __global__ void focal_loss_kernel(const float* __restrict__ z, const float* __re
 // Dropout (keras Dropout / SpatialDropout1D on (B,1,D) field embeddings == element-wise): counter-based
 // mask, so forward and backward regenerate the same bits from (seed, element index); nothing is stored.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t mix32(uint64_t x) {
-  x ^= x >> 33; x *= 0xff51afd7ed558ccdULL;
-  x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ULL;
-  x ^= x >> 33;
-  return (uint32_t)x;
+__global__ void dropout_kernel(const float* __restrict__ X, float* __restrict__ Y, int64_t n, uint32_t threshold,
+                               float scale, uint64_t seed, const unsigned long long* __restrict__ seed_dev) {
+  const uint64_t key = dropout_key(seed, seed_dev);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    Y[i] = mix32(key + (uint64_t)i) >= threshold ? X[i] * scale : 0.f;
 }
 
-__global__ void dropout_kernel(const float* __restrict__ X, float* __restrict__ Y, int64_t n, uint32_t threshold,
-                               float scale, uint64_t seed) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    Y[i] = mix32(seed * 0x9E3779B97F4A7C15ULL + (uint64_t)i) >= threshold ? X[i] * scale : 0.f;
+// end of a captured train step: every dropout call site's seed moves on by the number of sites, as the host's
+// counter does between two passes (48-bit wrap of deepmodel._Scope.next_seed)
+__global__ void seed_advance_kernel(unsigned long long* seeds, int n) {
+  for (int k = 0; k < n; ++k) seeds[k] = (seeds[k] + (unsigned long long)n) & 0xFFFFFFFFFFFFULL;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -575,12 +575,30 @@ int dtb_focal_loss_fwd_bwd(const float* z, const float* y_true, float* prob, flo
   return DTB_OK;
 }
 
+static int dropout_impl(const float* X, float* Y, int64_t n, float rate, unsigned long long seed,
+                        const unsigned long long* seed_dev, void* stream) {
+  if (n <= 0) return DTB_OK;
+  dropout_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(X, Y, n, dropout_threshold(rate), 1.f / (1.f - rate), seed,
+                                                               seed_dev);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
+
 int dtb_dropout(const float* X, float* Y, int64_t n, float rate, unsigned long long seed, void* stream) {
   DTB_CHECK_ARG(X && Y, "NULL argument");
   DTB_CHECK_ARG(rate >= 0.f && rate < 1.f, "rate must be in [0, 1)");
-  if (n <= 0) return DTB_OK;
-  const uint32_t threshold = (uint32_t)((double)rate * 4294967296.0);
-  dropout_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(X, Y, n, threshold, 1.f / (1.f - rate), seed);
+  return dropout_impl(X, Y, n, rate, seed, nullptr, stream);
+}
+
+int dtb_dropout_dev(const float* X, float* Y, int64_t n, float rate, const unsigned long long* seed, void* stream) {
+  DTB_CHECK_ARG(X && Y && seed, "NULL argument");
+  DTB_CHECK_ARG(rate >= 0.f && rate < 1.f, "rate must be in [0, 1)");
+  return dropout_impl(X, Y, n, rate, 0, seed, stream);
+}
+
+int dtb_seed_advance(unsigned long long* seeds, int n, void* stream) {
+  DTB_CHECK_ARG(seeds && n >= 1, "need a seed buffer of n >= 1 slots");
+  seed_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(seeds, n);
   DTB_LAUNCH_OK();
   return DTB_OK;
 }

@@ -70,6 +70,21 @@ __device__ __forceinline__ void red_add_f4(float* p, float4 v) {
                : "memory");
 }
 
+// Counter-based dropout masks (dense_bn_loss.cu, pnn_attention.cu): element i of a call with seed s is kept when
+// mix32(dropout_key(s) + i) >= threshold, threshold = rate * 2^32; forward and backward regenerate the same bits and
+// nothing is stored.  The seed is a kernel argument, or is read from device memory when seed_dev is set (a train step
+// captured in a CUDA graph must not bake the host's seed into its kernel arguments).
+__device__ __forceinline__ uint32_t mix32(uint64_t x) {
+  x ^= x >> 33; x *= 0xff51afd7ed558ccdULL;
+  x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ULL;
+  x ^= x >> 33;
+  return (uint32_t)x;
+}
+__device__ __forceinline__ uint64_t dropout_key(uint64_t seed, const unsigned long long* __restrict__ seed_dev) {
+  return (seed_dev ? (uint64_t)*seed_dev : seed) * 0x9E3779B97F4A7C15ULL;
+}
+static inline uint32_t dropout_threshold(float rate) { return (uint32_t)((double)rate * 4294967296.0); }
+
 // Row base (in floats) of categorical id `id` of field f, or -1 when out of range.
 __device__ __forceinline__ int64_t table_row(const int64_t* __restrict__ row_offsets, int f, int id,
                                              int D, int* status) {

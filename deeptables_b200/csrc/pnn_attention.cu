@@ -524,14 +524,43 @@ __global__ void __launch_bounds__(256) pnn_bwd_dk_t_kernel(const int32_t* __rest
 // ------------------------------------------------------------------------------------------
 // attention core.  qkvr: [B, F, 4*D] = relu projections [Q | K | V | R] of each field row.
 // One CTA per batch row; thread = (head, field).
+//
+// Attention dropout (reference layers.py:135-143, DROP = true): in training each softmax weight is kept with
+// probability 1 - rate and scaled by 1 / (1 - rate).  The weight of (batch row b, head h, query field q, key field k)
+// has the element index
+//     i = ((b * heads + h) * F + q) * F + k          (b counted from AttDrop::row0)
+// and is kept when mix32(dropout_key(seed) + i) >= rate * 2^32, the mask of dropout_kernel.  The index depends neither
+// on the batch size nor on how a launch groups batch rows per CTA, so a batch and its slices draw the same bits.  The
+// backward regenerates the mask: with w = softmax, m = 0 or 1 / (1 - rate) and w' = w m,
+//     dV = w'^T dout,   dw = (dout V^T) m,   ds = w (dw - sum_k dw w);
+// no mask and no extra activation is stored.
 // ------------------------------------------------------------------------------------------
 constexpr int kMaxDh = 64;
 
-__global__ void attention_core_fwd_kernel(const float* __restrict__ qkvr, float* __restrict__ Y, int B, int F, int D,
-                                          int heads, int use_res) {
+struct AttDrop {
+  uint32_t threshold;                    // rate * 2^32
+  float scale;                           // 1 / (1 - rate)
+  uint64_t seed;
+  const unsigned long long* seed_dev;    // non-null: the seed is read from device memory
+  int64_t row0;                          // index of the call's first batch row in the mask
+};
+
+// counter of weight (b, h, q, 0); the key fields follow at + k
+__device__ __forceinline__ uint64_t att_counter(const AttDrop& dr, uint64_t key, int b, int heads, int h, int F, int q) {
+  return key + (((uint64_t)(dr.row0 + b) * heads + h) * F + q) * F;
+}
+// factor of the weight at counter c: 0 or 1 / (1 - rate)
+__device__ __forceinline__ float att_keep(const AttDrop& dr, uint64_t c) {
+  return mix32(c) >= dr.threshold ? dr.scale : 0.f;
+}
+
+template <bool DROP>
+__device__ __forceinline__ void attention_core_fwd_body(const float* __restrict__ qkvr, float* __restrict__ Y, int B, int F,
+                                                        int D, int heads, int use_res, const AttDrop& dr) {
   extern __shared__ float sm[];     // [F][4D]
   const int dh = D / heads;
   const float scale = rsqrtf((float)dh);
+  const uint64_t key = DROP ? dropout_key(dr.seed, dr.seed_dev) : 0;
   for (int b = blockIdx.x; b < B; b += gridDim.x) {
     __syncthreads();
     const float* src = qkvr + (size_t)b * F * 4 * D;
@@ -551,6 +580,7 @@ __global__ void attention_core_fwd_kernel(const float* __restrict__ qkvr, float*
       float sum = 0.f;
       float acc[kMaxDh];
       for (int c = 0; c < dh; ++c) acc[c] = 0.f;
+      const uint64_t ctr = DROP ? att_counter(dr, key, b, heads, h, F, i) : 0;
       for (int j = 0; j < F; ++j) {
         const float* k = sm + (size_t)j * 4 * D + D + h * dh;
         const float* v = sm + (size_t)j * 4 * D + 2 * D + h * dh;
@@ -558,6 +588,7 @@ __global__ void attention_core_fwd_kernel(const float* __restrict__ qkvr, float*
         for (int c = 0; c < dh; ++c) s += q[c] * k[c];
         const float pj = __expf(s * scale - m);
         sum += pj;
+        if (DROP && att_keep(dr, ctr + j) == 0.f) continue;      // the 1 / (1 - rate) of the kept weights: below
         for (int c = 0; c < dh; ++c) acc[c] += pj * v[c];
       }
       const float inv = 1.f / sum;
@@ -565,6 +596,7 @@ __global__ void attention_core_fwd_kernel(const float* __restrict__ qkvr, float*
       const float* res = sm + (size_t)i * 4 * D + 3 * D + h * dh;
       for (int c = 0; c < dh; ++c) {
         float o = acc[c] * inv;
+        if (DROP) o *= dr.scale;
         if (use_res) o += res[c];
         y[c] = fmaxf(o, 0.f);
       }
@@ -572,10 +604,23 @@ __global__ void attention_core_fwd_kernel(const float* __restrict__ qkvr, float*
   }
 }
 
-__global__ void attention_core_bwd_kernel(const float* __restrict__ qkvr, const float* __restrict__ Y,
-                                          const float* __restrict__ dY, float* __restrict__ d_qkvr, int B, int F,
-                                          int D, int heads, int use_res, int mask_in) {
+// the kernels: the bodies above without dropout, under the names they have always had, and with it
+__global__ void attention_core_fwd_kernel(const float* __restrict__ qkvr, float* __restrict__ Y, int B, int F, int D,
+                                          int heads, int use_res) {
+  attention_core_fwd_body<false>(qkvr, Y, B, F, D, heads, use_res, AttDrop{});
+}
+__global__ void attention_core_dropout_fwd_kernel(const float* __restrict__ qkvr, float* __restrict__ Y, int B, int F,
+                                                  int D, int heads, int use_res, AttDrop dr) {
+  attention_core_fwd_body<true>(qkvr, Y, B, F, D, heads, use_res, dr);
+}
+
+template <bool DROP>
+__device__ __forceinline__ void attention_core_bwd_body(const float* __restrict__ qkvr, const float* __restrict__ Y,
+                                                        const float* __restrict__ dY, float* __restrict__ d_qkvr, int B,
+                                                        int F, int D, int heads, int use_res, int mask_in,
+                                                        const AttDrop& dr) {
   extern __shared__ float sm[];
+  const uint64_t key = DROP ? dropout_key(dr.seed, dr.seed_dev) : 0;
   float* blk = sm;                          // [F][4D] inputs
   float* dz = sm + (size_t)F * 4 * D;       // [F][D]   dLoss / d(pre-relu output)
   float* st = dz + (size_t)F * D;           // [heads*F][3]: max, 1/sum, delta
@@ -604,6 +649,7 @@ __global__ void attention_core_bwd_kernel(const float* __restrict__ qkvr, const 
         for (int c = 0; c < dh; ++c) s += q[c] * k[c];
         m = fmaxf(m, s * scale);
       }
+      const uint64_t ctr = DROP ? att_counter(dr, key, b, heads, h, F, i) : 0;
       float sum = 0.f, dsum = 0.f;       // dsum = sum_j p_j (dout . v_j)  (un-normalised)
       for (int j = 0; j < F; ++j) {
         const float* k = blk + (size_t)j * 4 * D + D + h * dh;
@@ -613,6 +659,7 @@ __global__ void attention_core_bwd_kernel(const float* __restrict__ qkvr, const 
           s += q[c] * k[c];
           dv += dout[c] * v[c];
         }
+        if (DROP) dv *= att_keep(dr, ctr + j);
         const float pj = __expf(s * scale - m);
         sum += pj;
         dsum += pj * dv;
@@ -632,6 +679,7 @@ __global__ void attention_core_bwd_kernel(const float* __restrict__ qkvr, const 
           s += q[c] * k[c];
           dv += dout[c] * v[c];
         }
+        if (DROP) dv *= att_keep(dr, ctr + j);
         const float ds = __expf(s * scale - m) * inv * (dv - delta);
         for (int c = 0; c < dh; ++c) dq[c] += ds * k[c];
       }
@@ -663,10 +711,16 @@ __global__ void attention_core_bwd_kernel(const float* __restrict__ qkvr, const 
           dv += dout[c] * v[c];
         }
         const float pij = __expf(s * scale - s3[0]) * s3[1];
+        float pm = pij;                 // the dropped weight w' = w m
+        if (DROP) {
+          const float mk = att_keep(dr, att_counter(dr, key, b, heads, h, F, i) + j);
+          dv *= mk;
+          pm *= mk;
+        }
         const float ds = pij * (dv - s3[2]);
         for (int c = 0; c < dh; ++c) {
           dk[c] += ds * q[c];
-          dvv[c] += pij * dout[c];
+          dvv[c] += pm * dout[c];
         }
       }
       float* o = dst + (size_t)j * 4 * D + h * dh;
@@ -676,6 +730,17 @@ __global__ void attention_core_bwd_kernel(const float* __restrict__ qkvr, const 
       }
     }
   }
+}
+
+__global__ void attention_core_bwd_kernel(const float* __restrict__ qkvr, const float* __restrict__ Y,
+                                          const float* __restrict__ dY, float* __restrict__ d_qkvr, int B, int F,
+                                          int D, int heads, int use_res, int mask_in) {
+  attention_core_bwd_body<false>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_res, mask_in, AttDrop{});
+}
+__global__ void attention_core_dropout_bwd_kernel(const float* __restrict__ qkvr, const float* __restrict__ Y,
+                                                  const float* __restrict__ dY, float* __restrict__ d_qkvr, int B, int F,
+                                                  int D, int heads, int use_res, int mask_in, AttDrop dr) {
+  attention_core_bwd_body<true>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_res, mask_in, dr);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -733,12 +798,13 @@ __device__ __forceinline__ void cp_async16(float* smem_dst, const void* gsrc) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-template <int DH>
-__global__ void __launch_bounds__(256) attention_core_fwd_t_kernel(const float* __restrict__ qkvr, float* __restrict__ Y, int B, int F, int D,
-                                                                    int heads, int use_res, int R, int nbuf) {
+template <int DH, bool DROP>
+__device__ __forceinline__ void attention_core_fwd_t_body(const float* __restrict__ qkvr, float* __restrict__ Y, int B, int F,
+                                                          int D, int heads, int use_res, int R, int nbuf, const AttDrop& dr) {
   extern __shared__ __align__(16) float sm_all[];     // [nbuf][R][F][4D + 4]
   const int RS = 4 * D + 4;
   const float scale = rsqrtf((float)DH);
+  const uint64_t key = DROP ? dropout_key(dr.seed, dr.seed_dev) : 0;
   const int hf = heads * F;
   const int rr = threadIdx.x / hf, t = threadIdx.x - rr * hf;       // batch row of the CTA's group, (head, field)
   const size_t buf_floats = (size_t)R * F * RS;
@@ -780,6 +846,7 @@ __global__ void __launch_bounds__(256) attention_core_fwd_t_kernel(const float* 
         m = fmaxf(m, s);
       }
       float sum = 0.f;
+      const uint64_t ctr = DROP ? att_counter(dr, key, b, heads, h, F, i) : 0;
       for (int j = 0; j < F; ++j) {
         const float* k = sm + (size_t)j * RS + D + h * DH;
         lds_row<DH>(k, kk);
@@ -787,8 +854,9 @@ __global__ void __launch_bounds__(256) attention_core_fwd_t_kernel(const float* 
         float s = 0.f;
 #pragma unroll
         for (int c = 0; c < DH; ++c) s = fmaf(q[c], kk[c], s);
-        const float pj = __expf(s - m);
+        float pj = __expf(s - m);
         sum += pj;
+        if (DROP && att_keep(dr, ctr + j) == 0.f) pj = 0.f;      // the 1 / (1 - rate) of the kept weights: below
 #pragma unroll
         for (int c = 0; c < DH; ++c) acc[c] = fmaf(pj, vv[c], acc[c]);
       }
@@ -797,6 +865,7 @@ __global__ void __launch_bounds__(256) attention_core_fwd_t_kernel(const float* 
 #pragma unroll
       for (int c = 0; c < DH; ++c) {
         float o = acc[c] * inv;
+        if (DROP) o *= dr.scale;
         if (use_res) o += vv[c];
         acc[c] = fmaxf(o, 0.f);
       }
@@ -812,11 +881,24 @@ __global__ void __launch_bounds__(256) attention_core_fwd_t_kernel(const float* 
 }
 
 template <int DH>
-__global__ void __launch_bounds__(256) attention_core_bwd_t_kernel(const float* __restrict__ qkvr, const float* __restrict__ Y,
-                                                                    const float* __restrict__ dY, float* __restrict__ d_qkvr, int B,
-                                                                    int F, int D, int heads, int use_res, int mask_in,
-                                                                    int R, int nbuf) {
+__global__ void __launch_bounds__(256) attention_core_fwd_t_kernel(const float* __restrict__ qkvr, float* __restrict__ Y, int B, int F, int D,
+                                                                    int heads, int use_res, int R, int nbuf) {
+  attention_core_fwd_t_body<DH, false>(qkvr, Y, B, F, D, heads, use_res, R, nbuf, AttDrop{});
+}
+template <int DH>
+__global__ void __launch_bounds__(256) attention_core_dropout_fwd_t_kernel(const float* __restrict__ qkvr, float* __restrict__ Y,
+                                                                            int B, int F, int D, int heads, int use_res, int R,
+                                                                            int nbuf, AttDrop dr) {
+  attention_core_fwd_t_body<DH, true>(qkvr, Y, B, F, D, heads, use_res, R, nbuf, dr);
+}
+
+template <int DH, bool DROP>
+__device__ __forceinline__ void attention_core_bwd_t_body(const float* __restrict__ qkvr, const float* __restrict__ Y,
+                                                          const float* __restrict__ dY, float* __restrict__ d_qkvr, int B,
+                                                          int F, int D, int heads, int use_res, int mask_in, int R, int nbuf,
+                                                          const AttDrop& dr) {
   extern __shared__ __align__(16) float sm_all[];
+  const uint64_t key = DROP ? dropout_key(dr.seed, dr.seed_dev) : 0;
   const int RS = 4 * D + 4, RZ = D + 4;
   const int hf = heads * F;
   const int rr = threadIdx.x / hf, t = threadIdx.x - rr * hf;       // batch row of the CTA's group, (head, field)
@@ -893,6 +975,7 @@ __global__ void __launch_bounds__(256) attention_core_bwd_t_kernel(const float* 
       float pk[DH];
 #pragma unroll
       for (int c = 0; c < DH; ++c) pk[c] = 0.f;
+      const uint64_t ctr = DROP ? att_counter(dr, key, b, heads, h, F, i) : 0;
       for (int j = 0; j < F; ++j) {
         const float* k = blk + (size_t)j * RS + D + h * DH;
         lds_row<DH>(k, kk);
@@ -903,6 +986,7 @@ __global__ void __launch_bounds__(256) attention_core_bwd_t_kernel(const float* 
           s = fmaf(q[c], kk[c], s);
           dv = fmaf(dout[c], vv[c], dv);
         }
+        if (DROP) dv *= att_keep(dr, ctr + j);
         const float pj = __expf(s - m);
         const float w = pj * dv;
         sum += pj;
@@ -942,6 +1026,7 @@ __global__ void __launch_bounds__(256) attention_core_bwd_t_kernel(const float* 
         dk[c] = 0.f;
         dvv[c] = 0.f;
       }
+      const uint64_t ctr = DROP ? att_counter(dr, key, b, heads, h, F, 0) + j : 0;     // weight (b, h, i, j) at + i * F
       for (int i = 0; i < F; ++i) {
         lds_row<DH>(blk + (size_t)i * RS + h * DH, q);
         lds_row<DH>(dz + (size_t)i * RZ + h * DH, dout);
@@ -953,11 +1038,17 @@ __global__ void __launch_bounds__(256) attention_core_bwd_t_kernel(const float* 
           dv = fmaf(dout[c], v[c], dv);
         }
         const float pij = __expf(s * scale - s3.x) * s3.y;
+        float pm = pij;                 // the dropped weight w' = w m
+        if (DROP) {
+          const float mk = att_keep(dr, ctr + (uint64_t)i * F);
+          dv *= mk;
+          pm *= mk;
+        }
         const float ds = pij * (dv - s3.z);
 #pragma unroll
         for (int c = 0; c < DH; ++c) {
           dk[c] = fmaf(ds, q[c], dk[c]);
-          dvv[c] = fmaf(pij, dout[c], dvv[c]);
+          dvv[c] = fmaf(pm, dout[c], dvv[c]);
         }
       }
       float* o = dst + (size_t)j * 4 * D + h * DH;
@@ -979,6 +1070,23 @@ __global__ void __launch_bounds__(256) attention_core_bwd_t_kernel(const float* 
       issue(b0n, 0);
     }
   }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(256) attention_core_bwd_t_kernel(const float* __restrict__ qkvr, const float* __restrict__ Y,
+                                                                    const float* __restrict__ dY, float* __restrict__ d_qkvr, int B,
+                                                                    int F, int D, int heads, int use_res, int mask_in,
+                                                                    int R, int nbuf) {
+  attention_core_bwd_t_body<DH, false>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_res, mask_in, R, nbuf, AttDrop{});
+}
+template <int DH>
+__global__ void __launch_bounds__(256) attention_core_dropout_bwd_t_kernel(const float* __restrict__ qkvr,
+                                                                            const float* __restrict__ Y,
+                                                                            const float* __restrict__ dY,
+                                                                            float* __restrict__ d_qkvr, int B, int F, int D,
+                                                                            int heads, int use_res, int mask_in, int R, int nbuf,
+                                                                            AttDrop dr) {
+  attention_core_bwd_t_body<DH, true>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_res, mask_in, R, nbuf, dr);
 }
 
 }  // namespace dtb
@@ -1006,6 +1114,123 @@ bool pnn_t_shape(int D, const void* table, const void* grad_table) {
   if (reinterpret_cast<uintptr_t>(table) & 15) return false;
   if (grad_table && (reinterpret_cast<uintptr_t>(grad_table) & 15)) return false;
   return true;
+}
+
+// the attention launches; DROP = false launches the kernels that hold no dropout code
+template <bool DROP>
+int attention_fwd(const float* qkvr, float* Y, int B, int F, int D, int heads, int use_residual, const AttDrop& dr,
+                  void* stream) {
+  if (B == 0) return DTB_OK;
+  const int threads = (heads * F + 31) / 32 * 32;
+  int grid = sm_count() * 8;
+  if (grid > B) grid = B;
+  const int dh = D / heads;
+  const int nthr = threads < 64 ? 64 : threads;
+  if (D % 4 == 0 && nthr <= 256 && ((reinterpret_cast<uintptr_t>(qkvr) | reinterpret_cast<uintptr_t>(Y)) & 15) == 0) {
+    const size_t row_bytes = (size_t)F * (4 * D + 4) * sizeof(float);
+    int R, nbuf;
+    att_plan(heads * F, row_bytes, 0, R, nbuf);
+    const int nthr_t = att_threads(R, heads * F);
+    const size_t smem_t = (size_t)nbuf * R * row_bytes;
+    if (grid > ceil_div(B, R)) grid = ceil_div(B, R);
+    if (smem_t <= kAttSmemMax) {
+#define DTB_ATT_FWD(DHV)                                                                                                 \
+  case DHV:                                                                                                              \
+    if constexpr (DROP) {                                                                                                \
+      DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_dropout_fwd_t_kernel<DHV>,                                         \
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_t));                       \
+      attention_core_dropout_fwd_t_kernel<DHV><<<grid, nthr_t, smem_t, (cudaStream_t)stream>>>(                          \
+          qkvr, Y, B, F, D, heads, use_residual, R, nbuf, dr);                                                           \
+    } else {                                                                                                             \
+      DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_fwd_t_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
+                                       (int)smem_t));                                                                    \
+      attention_core_fwd_t_kernel<DHV><<<grid, nthr_t, smem_t, (cudaStream_t)stream>>>(qkvr, Y, B, F, D, heads,          \
+                                                                                       use_residual, R, nbuf);           \
+    }                                                                                                                    \
+    DTB_LAUNCH_OK();                                                                                                     \
+    return DTB_OK;
+    switch (dh) {
+      DTB_ATT_FWD(1) DTB_ATT_FWD(2) DTB_ATT_FWD(4) DTB_ATT_FWD(8) DTB_ATT_FWD(16) DTB_ATT_FWD(32) DTB_ATT_FWD(64)
+      default: break;
+    }
+    }
+#undef DTB_ATT_FWD
+  }
+  const size_t smem = (size_t)F * 4 * D * sizeof(float);
+  if constexpr (DROP) {
+    DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_dropout_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
+    attention_core_dropout_fwd_kernel<<<grid, nthr, smem, (cudaStream_t)stream>>>(qkvr, Y, B, F, D, heads, use_residual,
+                                                                                  dr);
+  } else {
+    DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attention_core_fwd_kernel<<<grid, nthr, smem, (cudaStream_t)stream>>>(qkvr, Y, B, F, D, heads, use_residual);
+  }
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
+
+template <bool DROP>
+int attention_bwd(const float* qkvr, const float* Y, const float* dY, float* d_qkvr, int B, int F, int D, int heads,
+                  int use_residual, int mask_relu_inputs, const AttDrop& dr, void* stream) {
+  if (B == 0) return DTB_OK;
+  const int threads = (heads * F + 31) / 32 * 32;
+  int grid = sm_count() * 8;
+  if (grid > B) grid = B;
+  const int dh = D / heads;
+  const int nthr = threads < 64 ? 64 : threads;
+  if (D % 4 == 0 && nthr <= 256 &&
+      ((reinterpret_cast<uintptr_t>(qkvr) | reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(dY) |
+        reinterpret_cast<uintptr_t>(d_qkvr)) & 15) == 0) {
+    const size_t row_bytes = ((size_t)F * (4 * D + 4) + 2 * (size_t)F * (D + 4)) * sizeof(float);
+    const size_t stat_bytes = (size_t)heads * F * 4 * sizeof(float);
+    int R, nbuf;
+    att_plan(heads * F, row_bytes, stat_bytes, R, nbuf);
+    const int nthr_t = att_threads(R, heads * F);
+    const size_t smem_t = (size_t)R * (nbuf * row_bytes + stat_bytes);
+    if (grid > ceil_div(B, R)) grid = ceil_div(B, R);
+    if (smem_t <= kAttSmemMax) {
+#define DTB_ATT_BWD(DHV)                                                                                                 \
+  case DHV:                                                                                                              \
+    if constexpr (DROP) {                                                                                                \
+      DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_dropout_bwd_t_kernel<DHV>,                                         \
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_t));                       \
+      attention_core_dropout_bwd_t_kernel<DHV><<<grid, nthr_t, smem_t, (cudaStream_t)stream>>>(                          \
+          qkvr, Y, dY, d_qkvr, B, F, D, heads, use_residual, mask_relu_inputs, R, nbuf, dr);                             \
+    } else {                                                                                                             \
+      DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_bwd_t_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
+                                       (int)smem_t));                                                                    \
+      attention_core_bwd_t_kernel<DHV><<<grid, nthr_t, smem_t, (cudaStream_t)stream>>>(                                  \
+          qkvr, Y, dY, d_qkvr, B, F, D, heads, use_residual, mask_relu_inputs, R, nbuf);                                 \
+    }                                                                                                                    \
+    DTB_LAUNCH_OK();                                                                                                     \
+    return DTB_OK;
+    switch (dh) {
+      DTB_ATT_BWD(1) DTB_ATT_BWD(2) DTB_ATT_BWD(4) DTB_ATT_BWD(8) DTB_ATT_BWD(16) DTB_ATT_BWD(32)
+      default: break;
+    }
+    // heads of 64 already spill at 255 registers without dropout; with the mask's 64-bit counters on top ptxas gives up
+    // (32 registers, 10 KB of spill traffic per thread), so dropout at that width runs the any-shape kernel below
+    if constexpr (!DROP) switch (dh) {
+      DTB_ATT_BWD(64)
+      default: break;
+    }
+    }
+#undef DTB_ATT_BWD
+  }
+  const size_t smem = ((size_t)F * 5 * D + (size_t)heads * F * 3) * sizeof(float);
+  if constexpr (DROP) {
+    DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_dropout_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
+    attention_core_dropout_bwd_kernel<<<grid, nthr, smem, (cudaStream_t)stream>>>(qkvr, Y, dY, d_qkvr, B, F, D, heads,
+                                                                                  use_residual, mask_relu_inputs, dr);
+  } else {
+    DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attention_core_bwd_kernel<<<grid, nthr, smem, (cudaStream_t)stream>>>(qkvr, Y, dY, d_qkvr, B, F, D, heads,
+                                                                          use_residual, mask_relu_inputs);
+  }
+  DTB_LAUNCH_OK();
+  return DTB_OK;
 }
 }  // namespace
 
@@ -1122,91 +1347,47 @@ int dtb_pnn_bwd(const int32_t* idx, const float* table, const int64_t* row_offse
   return DTB_OK;
 }
 
+#define DTB_ATT_CHECK_SHAPE()                                                                                          \
+  DTB_CHECK_ARG(B >= 0 && F >= 1 && D >= 1 && heads >= 1 && D % heads == 0, "bad shape (num_heads must divide D)");     \
+  DTB_CHECK_ARG(D / heads <= kMaxDh && heads * F <= 1024, "head width <= 64 and heads*fields <= 1024")
+
 int dtb_attention_core_fwd(const float* qkvr, float* Y, int B, int F, int D, int heads, int use_residual,
                            void* stream) {
   DTB_CHECK_ARG(qkvr && Y, "NULL argument");
-  DTB_CHECK_ARG(B >= 0 && F >= 1 && D >= 1 && heads >= 1 && D % heads == 0, "bad shape (num_heads must divide D)");
-  DTB_CHECK_ARG(D / heads <= kMaxDh && heads * F <= 1024, "head width <= 64 and heads*fields <= 1024");
-  if (B == 0) return DTB_OK;
-  const int threads = (heads * F + 31) / 32 * 32;
-  int grid = sm_count() * 8;
-  if (grid > B) grid = B;
-  const int dh = D / heads;
-  const int nthr = threads < 64 ? 64 : threads;
-  if (D % 4 == 0 && nthr <= 256 && ((reinterpret_cast<uintptr_t>(qkvr) | reinterpret_cast<uintptr_t>(Y)) & 15) == 0) {
-    const size_t row_bytes = (size_t)F * (4 * D + 4) * sizeof(float);
-    int R, nbuf;
-    att_plan(heads * F, row_bytes, 0, R, nbuf);
-    const int nthr_t = att_threads(R, heads * F);
-    const size_t smem_t = (size_t)nbuf * R * row_bytes;
-    if (grid > ceil_div(B, R)) grid = ceil_div(B, R);
-    if (smem_t <= kAttSmemMax) {
-#define DTB_ATT_FWD(DHV)                                                                                                   \
-  case DHV:                                                                                                                \
-    DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_fwd_t_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
-                                     (int)smem_t));                                                                         \
-    attention_core_fwd_t_kernel<DHV><<<grid, nthr_t, smem_t, (cudaStream_t)stream>>>(qkvr, Y, B, F, D, heads,            \
-                                                                                     use_residual, R, nbuf);             \
-    DTB_LAUNCH_OK();                                                                                                       \
-    return DTB_OK;
-    switch (dh) {
-      DTB_ATT_FWD(1) DTB_ATT_FWD(2) DTB_ATT_FWD(4) DTB_ATT_FWD(8) DTB_ATT_FWD(16) DTB_ATT_FWD(32) DTB_ATT_FWD(64)
-      default: break;
-    }
-    }
-#undef DTB_ATT_FWD
-  }
-  const size_t smem = (size_t)F * 4 * D * sizeof(float);
-  DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  attention_core_fwd_kernel<<<grid, nthr, smem, (cudaStream_t)stream>>>(qkvr, Y, B, F, D, heads, use_residual);
-  DTB_LAUNCH_OK();
-  return DTB_OK;
+  DTB_ATT_CHECK_SHAPE();
+  return attention_fwd<false>(qkvr, Y, B, F, D, heads, use_residual, AttDrop{}, stream);
 }
 
 int dtb_attention_core_bwd(const float* qkvr, const float* Y, const float* dY, float* d_qkvr, int B, int F, int D,
                            int heads, int use_residual, int mask_relu_inputs, void* stream) {
   DTB_CHECK_ARG(qkvr && Y && dY && d_qkvr, "NULL argument");
-  DTB_CHECK_ARG(B >= 0 && F >= 1 && D >= 1 && heads >= 1 && D % heads == 0, "bad shape (num_heads must divide D)");
-  DTB_CHECK_ARG(D / heads <= kMaxDh && heads * F <= 1024, "head width <= 64 and heads*fields <= 1024");
-  if (B == 0) return DTB_OK;
-  const int threads = (heads * F + 31) / 32 * 32;
-  int grid = sm_count() * 8;
-  if (grid > B) grid = B;
-  const int dh = D / heads;
-  const int nthr = threads < 64 ? 64 : threads;
-  if (D % 4 == 0 && nthr <= 256 &&
-      ((reinterpret_cast<uintptr_t>(qkvr) | reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(dY) |
-        reinterpret_cast<uintptr_t>(d_qkvr)) & 15) == 0) {
-    const size_t row_bytes = ((size_t)F * (4 * D + 4) + 2 * (size_t)F * (D + 4)) * sizeof(float);
-    const size_t stat_bytes = (size_t)heads * F * 4 * sizeof(float);
-    int R, nbuf;
-    att_plan(heads * F, row_bytes, stat_bytes, R, nbuf);
-    const int nthr_t = att_threads(R, heads * F);
-    const size_t smem_t = (size_t)R * (nbuf * row_bytes + stat_bytes);
-    if (grid > ceil_div(B, R)) grid = ceil_div(B, R);
-    if (smem_t <= kAttSmemMax) {
-#define DTB_ATT_BWD(DHV)                                                                                                \
-  case DHV:                                                                                                             \
-    DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_bwd_t_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                     (int)smem_t));                                                                      \
-    attention_core_bwd_t_kernel<DHV><<<grid, nthr_t, smem_t, (cudaStream_t)stream>>>(qkvr, Y, dY, d_qkvr, B, F, D,      \
-                                                                                     heads, use_residual,                \
-                                                                                     mask_relu_inputs, R, nbuf);         \
-    DTB_LAUNCH_OK();                                                                                                    \
-    return DTB_OK;
-    switch (dh) {
-      DTB_ATT_BWD(1) DTB_ATT_BWD(2) DTB_ATT_BWD(4) DTB_ATT_BWD(8) DTB_ATT_BWD(16) DTB_ATT_BWD(32) DTB_ATT_BWD(64)
-      default: break;
-    }
-    }
-#undef DTB_ATT_BWD
-  }
-  const size_t smem = ((size_t)F * 5 * D + (size_t)heads * F * 3) * sizeof(float);
-  DTB_CUDA_OK(cudaFuncSetAttribute(attention_core_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  attention_core_bwd_kernel<<<grid, nthr, smem, (cudaStream_t)stream>>>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_residual,
-                                                                        mask_relu_inputs);
-  DTB_LAUNCH_OK();
-  return DTB_OK;
+  DTB_ATT_CHECK_SHAPE();
+  return attention_bwd<false>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_residual, mask_relu_inputs, AttDrop{}, stream);
 }
+
+int dtb_attention_core_dropout_fwd(const float* qkvr, float* Y, int B, int F, int D, int heads, int use_residual,
+                                   float rate, unsigned long long seed, const unsigned long long* seed_dev,
+                                   long long row_offset, void* stream) {
+  DTB_CHECK_ARG(qkvr && Y, "NULL argument");
+  DTB_ATT_CHECK_SHAPE();
+  DTB_CHECK_ARG(rate >= 0.f && rate < 1.f && row_offset >= 0, "rate must be in [0, 1), row_offset >= 0");
+  if (rate == 0.f) return attention_fwd<false>(qkvr, Y, B, F, D, heads, use_residual, AttDrop{}, stream);
+  const AttDrop dr{dropout_threshold(rate), 1.f / (1.f - rate), seed, seed_dev, row_offset};
+  return attention_fwd<true>(qkvr, Y, B, F, D, heads, use_residual, dr, stream);
+}
+
+int dtb_attention_core_dropout_bwd(const float* qkvr, const float* Y, const float* dY, float* d_qkvr, int B, int F,
+                                   int D, int heads, int use_residual, int mask_relu_inputs, float rate,
+                                   unsigned long long seed, const unsigned long long* seed_dev, long long row_offset,
+                                   void* stream) {
+  DTB_CHECK_ARG(qkvr && Y && dY && d_qkvr, "NULL argument");
+  DTB_ATT_CHECK_SHAPE();
+  DTB_CHECK_ARG(rate >= 0.f && rate < 1.f && row_offset >= 0, "rate must be in [0, 1), row_offset >= 0");
+  if (rate == 0.f)
+    return attention_bwd<false>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_residual, mask_relu_inputs, AttDrop{}, stream);
+  const AttDrop dr{dropout_threshold(rate), 1.f / (1.f - rate), seed, seed_dev, row_offset};
+  return attention_bwd<true>(qkvr, Y, dY, d_qkvr, B, F, D, heads, use_residual, mask_relu_inputs, dr, stream);
+}
+#undef DTB_ATT_CHECK_SHAPE
 
 }  // extern "C"

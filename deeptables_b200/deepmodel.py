@@ -29,6 +29,9 @@ from ._native import ptr, check, stream_ptr
 from . import _native as N
 
 
+SEED_MASK = 0xFFFFFFFFFFFF
+
+
 class _Scope:
     """Active-forward-pass state: parameter store + Keras-style layer naming."""
 
@@ -50,11 +53,53 @@ class _Scope:
         self._indices = {}
         self._prefix = []
         self._seed_counter = 0
+        self.seed_sites = 0                # dropout call sites of one training pass (counted by every train step)
+        self._seed_dev = None              # int64[seed_sites] (values < 2^48): the seeds a captured train step reads
+        self._seed_dev_at = None           # the _seed_counter those values belong to
+        self._slots = None                 # inside device_seeds(): slots handed out so far
+
+    def seed_at(self, counter):
+        return (int(self.generator.initial_seed()) * 1000003 + counter) & SEED_MASK
 
     def next_seed(self):
-        """Fresh dropout seed per call site and per pass (drawn from the model's generator stream)."""
+        """Fresh dropout seed per call site and per pass (drawn from the model's generator stream): an integer, or
+        inside device_seeds() the device slot that holds that integer when the captured step runs."""
         self._seed_counter += 1
-        return (int(self.generator.initial_seed()) * 1000003 + self._seed_counter) & 0xFFFFFFFFFFFF
+        if self._slots is not None:
+            self._slots += 1
+            return self._seed_dev[self._slots - 1:self._slots]
+        return self.seed_at(self._seed_counter)
+
+    def slot_seeds(self):
+        """What the device slots hold before a training pass that starts at the current counter: the integers
+        next_seed() would return during it, in call order."""
+        return [self.seed_at(self._seed_counter + 1 + k) for k in range(self.seed_sites)]
+
+    @contextlib.contextmanager
+    def device_seeds(self):
+        """Around the capture of a train step in a CUDA graph: next_seed() hands out slots of the device seed buffer
+        (allocated once: its address is captured) and the counter is put back, as a capture runs nothing.  Yields
+        the buffer, None for a model without dropout."""
+        if self._seed_dev is None and self.seed_sites:
+            self._seed_dev = torch.zeros(self.seed_sites, dtype=torch.int64, device=self.device)
+        start, self._slots = self._seed_counter, 0
+        try:
+            yield self._seed_dev
+            if self._slots != self.seed_sites:
+                raise RuntimeError(f'{self._slots} dropout call sites in the captured pass, {self.seed_sites} before')
+        finally:
+            self._seed_counter, self._slots = start, None
+
+    def replay_seeds(self):
+        """Before a replay of the captured step: the device slots hold this pass's seeds (written here unless the last
+        replay's dtb_seed_advance left them so) and the host counter moves past them, as the replay's own
+        dtb_seed_advance moves the slots."""
+        if not self.seed_sites:
+            return
+        if self._seed_dev_at != self._seed_counter:
+            self._seed_dev.copy_(torch.tensor(self.slot_seeds(), dtype=torch.int64))
+        self._seed_counter += self.seed_sites
+        self._seed_dev_at = self._seed_counter
 
     def _begin_pass(self):
         self._counters = {}
@@ -367,8 +412,8 @@ class DeepModel:
                 block = E.FieldBlock(cat, self.table)
                 if cfg.embedding_dropout > 0 and training:
                     # SpatialDropout1D per field (reference layers.py:878-901): the mask must be shared by
-                    # every consumer, so this (non-default-for-benchmarks) mode materialises the dropped
-                    # block once and feeds the same fused kernels through the tensor-backed table facade
+                    # every consumer, so this mode materialises the dropped block once and feeds the same
+                    # fused kernels through the tensor-backed table facade
                     dropped = E.DropoutFn.apply(block.materialize(), cfg.embedding_dropout, scope.next_seed())
                     block = E.FieldBlock.from_tensor(dropped)
                 embeddings = E.EmbeddingList(block)
@@ -514,9 +559,11 @@ class DeepModel:
         """forward + loss + backward + (DP exchange) + Adam on one device-resident batch.
         Returns the batch predictions; the summed loss accumulates in ``self._loss_acc``.
 
-        Single-GPU steps without dropout or sample weights are captured ONCE per batch shape in a CUDA graph and replayed
+        Single-GPU steps without sample weights are captured ONCE per batch shape in a CUDA graph and replayed
         (``DTB_CUDA_GRAPH=0`` disables it): a step is ~90 launches of kernels that take microseconds at small batch sizes
-        (DeepFM at 8 192 rows), where the host's launch path -- not the GPU -- would set the pace."""
+        (DeepFM at 8 192 rows), where the host's launch path -- not the GPU -- would set the pace.  Dropout seeds, like
+        the step counter and the rate table, are read from device memory by a captured step (``_Scope.device_seeds``):
+        every step draws the seeds it would draw eagerly."""
         # the table covers this step before the table optimiser is chosen for it; a rate that overflowed is refused
         # before anything runs
         if self._rates.ensure(self._step + 1):
@@ -541,7 +588,9 @@ class DeepModel:
             t.pending_bwd = 0
             t.on_grad_final = (lambda: self._begin_table_exchange(cat)) if (self._dist and t.lazy_adam) else None
         self._early_exchange = None
+        seeds_before = scope._seed_counter
         z = self._forward(cat, cont, training=True)
+        scope.seed_sites = scope._seed_counter - seeds_before
         prob, dz = E.loss_forward_backward(z, y, self.task, sample_weight, True, self._loss_acc, focal=self._focal)
         dp.scale_for_mean(dz)
         z.backward(dz)
@@ -641,21 +690,16 @@ class DeepModel:
                                      float(loss_scale), stream_ptr()), 'reg_grad(table)')
 
     # ---- CUDA-graph replay of the train step ---------------------------------------------------------------------------
-    def _has_dropout(self):
-        cfg = self.config
-        if cfg.embedding_dropout or cfg.dense_dropout:
-            return True
-        if any(float(u[1]) > 0 for u in (cfg.dnn_params or {}).get('hidden_units', ())):
-            return True
-        return bool((cfg.autoint_params or {}).get('dropout_rate', 0)) and 'autoint_nets' in cfg.nets
-
     def _graph_eligible(self, cat, cont, y, sample_weight):
         if self._dist or sample_weight is not None or os.environ.get('DTB_CUDA_GRAPH', '1') == '0':
             return False
         if self._graph_failed or self._step < 1:       # the first step runs eagerly (allocations, lazy initialisation)
             return False
         if getattr(self, '_no_graph', None) is None:
-            self._no_graph = self._has_dropout() or any(callable(n) for n in self.config.nets)
+            # per-column embedding widths with embedding dropout: the dropped flat block feeds the nets through
+            # slices, a path that has only run eagerly (tests/test_widths_gpu.py expects eager launches there)
+            ragged_dropout = self.table is not None and self.table.ragged and self.config.embedding_dropout > 0
+            self._no_graph = ragged_dropout or any(callable(n) for n in self.config.nets)
         return not self._no_graph
 
     def _train_step_graphed(self, cat, cont, y):
@@ -682,8 +726,10 @@ class DeepModel:
                 torch.cuda.synchronize()
                 graph = torch.cuda.CUDAGraph()
                 l0 = N.lib.dtb_launch_count()
-                with torch.cuda.graph(graph):
+                with self._scope.device_seeds() as seeds, torch.cuda.graph(graph):
                     prob = self._train_step_body(sc, sx, sy, None, dev_step=True)
+                    if seeds is not None:
+                        check(N.lib.dtb_seed_advance(ptr(seeds), seeds.numel(), stream_ptr()), 'seed_advance')
                 n_launch = N.lib.dtb_launch_count() - l0          # kernels of this library inside one replay
             except Exception as exc:                       # capture unsupported here: say so once, run eagerly from now on
                 self._graph_failed = True
@@ -702,6 +748,7 @@ class DeepModel:
         if sx is not None:
             sx.copy_(cont)
         sy.copy_(y)
+        self._scope.replay_seeds()
         graph.replay()
         N.lib.dtb_launch_count_add(n_launch)
         self._step += 1

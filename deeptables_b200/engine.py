@@ -435,6 +435,20 @@ def batchnorm_infer(x, gamma, beta, moving_mean, moving_var):
     return y
 
 
+def _seed_args(seed):
+    """(host seed, device seed pointer) of a dropout seed: an integer, or inside the capture of a CUDA graph the
+    one-element device slot ``_Scope.next_seed`` hands out."""
+    return (0, ptr(seed)) if torch.is_tensor(seed) else (int(seed), None)
+
+
+def _dropout(x, y, rate, seed, what):
+    host, dev = _seed_args(seed)
+    if dev is not None:
+        check(N.lib.dtb_dropout_dev(ptr(x), ptr(y), x.numel(), rate, dev, stream_ptr()), what)
+    else:
+        check(N.lib.dtb_dropout(ptr(x), ptr(y), x.numel(), rate, host, stream_ptr()), what)
+
+
 class DropoutFn(torch.autograd.Function):
     """keras Dropout / SpatialDropout1D on field embeddings: counter-based mask, nothing stored."""
 
@@ -442,15 +456,15 @@ class DropoutFn(torch.autograd.Function):
     def forward(ctx, x, rate, seed):
         x = _f32(x)
         y = torch.empty_like(x)
-        check(N.lib.dtb_dropout(ptr(x), ptr(y), x.numel(), float(rate), int(seed), stream_ptr()), 'dropout')
-        ctx.cfg = (float(rate), int(seed))
+        _dropout(x, y, float(rate), seed, 'dropout')
+        ctx.cfg = (float(rate), seed)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         dy = _f32(dy)
         dx = torch.empty_like(dy)
-        check(N.lib.dtb_dropout(ptr(dy), ptr(dx), dy.numel(), ctx.cfg[0], ctx.cfg[1], stream_ptr()), 'dropout_bwd')
+        _dropout(dy, dx, ctx.cfg[0], ctx.cfg[1], 'dropout_bwd')
         return dx, None, None
 
 
@@ -774,31 +788,42 @@ class MaxPoolFieldsFn(torch.autograd.Function):
 
 class AttentionCoreFn(torch.autograd.Function):
     """MultiheadAttention.call between the projections and the BatchNormalization
-    (layers.py:129-150): per-head softmax(QK^T/sqrt(dh))V + residual, relu."""
+    (layers.py:129-150): per-head softmax(QK^T/sqrt(dh))V + residual, relu; with ``rate`` > 0 dropout on the softmax
+    weights, its mask regenerated in backward from ``seed``."""
 
     @staticmethod
-    def forward(ctx, qkvr, heads, use_residual, mask_inputs=False):
+    def forward(ctx, qkvr, heads, use_residual, mask_inputs=False, rate=0.0, seed=None):
         """mask_inputs: qkvr are relu outputs and backward returns the gradient of their pre-activations."""
         qkvr = _f32(qkvr)
         b, f, d4 = qkvr.shape
         d = d4 // 4
         y = torch.empty(b, f, d, dtype=torch.float32, device=qkvr.device)
-        check(N.lib.dtb_attention_core_fwd(ptr(qkvr), ptr(y), b, f, d, heads, int(use_residual), stream_ptr()),
-              'attention_core_fwd')
+        rate = float(rate)
+        if rate > 0:
+            check(N.lib.dtb_attention_core_dropout_fwd(ptr(qkvr), ptr(y), b, f, d, heads, int(use_residual), rate,
+                                                       *_seed_args(seed), 0, stream_ptr()), 'attention_core_dropout_fwd')
+        else:
+            check(N.lib.dtb_attention_core_fwd(ptr(qkvr), ptr(y), b, f, d, heads, int(use_residual), stream_ptr()),
+                  'attention_core_fwd')
         ctx.save_for_backward(qkvr, y)
-        ctx.cfg = (heads, int(use_residual), int(bool(mask_inputs)))
+        ctx.cfg = (heads, int(use_residual), int(bool(mask_inputs)), rate, seed)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         qkvr, y = ctx.saved_tensors
         b, f, d4 = qkvr.shape
-        heads, use_res, mask = ctx.cfg
+        heads, use_res, mask, rate, seed = ctx.cfg
         dy = _f32(dy)
         dq = torch.empty_like(qkvr)
-        check(N.lib.dtb_attention_core_bwd(ptr(qkvr), ptr(y), ptr(dy), ptr(dq), b, f, d4 // 4, heads, use_res, mask,
-                                           stream_ptr()), 'attention_core_bwd')
-        return dq, None, None, None
+        if rate > 0:
+            check(N.lib.dtb_attention_core_dropout_bwd(ptr(qkvr), ptr(y), ptr(dy), ptr(dq), b, f, d4 // 4, heads, use_res,
+                                                       mask, rate, *_seed_args(seed), 0, stream_ptr()),
+                  'attention_core_dropout_bwd')
+        else:
+            check(N.lib.dtb_attention_core_bwd(ptr(qkvr), ptr(y), ptr(dy), ptr(dq), b, f, d4 // 4, heads, use_res, mask,
+                                               stream_ptr()), 'attention_core_bwd')
+        return dq, None, None, None, None, None
 
 
 TASK_CODES = {'binary': 0, 'multilabel': 0, 'regression': 1, 'multiclass': 2}

@@ -332,8 +332,8 @@ class MultiheadAttention(Layer):
         self.num_heads = params.get('num_heads', 1)
         self.dropout_rate = params.get('dropout_rate', 0)
         self.use_residual = params.get('use_residual', True)
-        if self.dropout_rate:
-            raise NotImplementedError('attention dropout_rate > 0 is not supported')
+        if not 0 <= self.dropout_rate < 1:
+            raise ValueError(f'Invalid value {self.dropout_rate} received for `rate`, expected a value in [0, 1).')
 
     def call(self, scope, x):
         x = _materialize(x)
@@ -350,7 +350,11 @@ class MultiheadAttention(Layer):
         # the attention backward has the relu outputs in shared memory and applies their mask itself, so the [B*F, 4D]
         # activation-gradient pass (and the gradient clone it needs) of the projection layer is skipped
         qkvr = E.DenseFn.apply(x, torch.cat(ws, dim=1), torch.cat(bs), E.ACT_CODES['relu'], True)
-        out = E.AttentionCoreFn.apply(qkvr, int(self.num_heads), bool(self.use_residual), True)
+        if self.dropout_rate > 0 and scope.training:        # on the softmax weights, inside the attention kernels
+            out = E.AttentionCoreFn.apply(qkvr, int(self.num_heads), bool(self.use_residual), True,
+                                          float(self.dropout_rate), scope.next_seed())
+        else:
+            out = E.AttentionCoreFn.apply(qkvr, int(self.num_heads), bool(self.use_residual), True)
         with scope.name_prefix(self.name):
             return BatchNormalization(name='batch_normalize')(out)
 

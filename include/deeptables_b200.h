@@ -130,6 +130,11 @@ int dtb_dense_bwd(const float* X, const float* W, const float* Y, float* dY, flo
 /* Y[i] = keep(seed, i) ? X[i]/(1-rate) : 0 with a counter-based mask: calling it again on dLoss/dY with
  * the same seed IS the backward.  Y may alias X. */
 int dtb_dropout(const float* X, float* Y, int64_t n, float rate, unsigned long long seed, void* stream);
+/* CUDA-graph forms: the seed is read from DEVICE memory, so a captured train step replays with a fresh mask: same
+ * bits as dtb_dropout for the same seed value.  dtb_seed_advance, once at the end of the captured step, moves each of
+ * the step's n seeds (one per dropout call site) on by n, modulo 2^48. */
+int dtb_dropout_dev(const float* X, float* Y, int64_t n, float rate, const unsigned long long* seed, void* stream);
+int dtb_seed_advance(unsigned long long* seeds, int n, void* stream);
 
 /* ---- losses on the task_output pre-activation (deepmodel.py:319-346, 436-457) ------------ */
 /* task: 0 binary/multilabel (sigmoid + BCE, probabilities clipped to [1e-7,1-1e-7] as keras),
@@ -413,6 +418,19 @@ int dtb_attention_core_fwd(const float* qkvr, float* Y, int B, int F, int D, int
 int dtb_attention_core_bwd(const float* qkvr, const float* Y, const float* dY, float* d_qkvr, int B,
                            int F, int D, int heads, int use_residual, int mask_relu_inputs,
                            void* stream);
+/* The same with dropout on the softmax weights (layers.py:111,141; training only): weight (b, h, q, k) -- batch row,
+ * head, query field, key field -- is kept with probability 1 - rate and scaled by 1 / (1 - rate).  The mask is that of
+ * dtb_dropout at element index ((b * heads + h) * F + q) * F + k, with b counted from row_offset (a slice of a batch
+ * that starts at row r and passes row_offset = r draws the bits of the whole batch).  The backward regenerates it:
+ * nothing is stored.  The seed is *seed_dev when seed_dev is not NULL (CUDA-graph form), else `seed`.  rate = 0 runs
+ * the kernels of dtb_attention_core_fwd/bwd. */
+int dtb_attention_core_dropout_fwd(const float* qkvr, float* Y, int B, int F, int D, int heads, int use_residual,
+                                   float rate, unsigned long long seed, const unsigned long long* seed_dev,
+                                   long long row_offset, void* stream);
+int dtb_attention_core_dropout_bwd(const float* qkvr, const float* Y, const float* dY, float* d_qkvr, int B, int F,
+                                   int D, int heads, int use_residual, int mask_relu_inputs, float rate,
+                                   unsigned long long seed, const unsigned long long* seed_dev, long long row_offset,
+                                   void* stream);
 
 #ifdef __cplusplus
 }
