@@ -34,6 +34,17 @@ class OptimParams(ctypes.Structure):
 OPTIM_SGD, OPTIM_RMSPROP, OPTIM_ADAGRAD = 1, 2, 3
 _OPP = POINTER(OptimParams)
 
+METRIC_MAX_LISTS, METRIC_MAX_THRESHOLDS = 8, 2048
+
+
+class MetricPlan(ctypes.Structure):
+    """``dtb_metric_plan`` (host memory, read at call time): what one ``dtb_metrics_update`` accumulates."""
+    _fields_ = [('cols', c_int), ('n_lists', c_int), ('list_len', c_int * METRIC_MAX_LISTS),
+                ('list_off', c_int * METRIC_MAX_LISTS), ('sums', c_int), ('argmax', c_int), ('top_k', c_int)]
+
+
+_MPP = POINTER(MetricPlan)
+
 _SIGNATURES = {
     'dtb_version': (c_int, []),
     'dtb_last_error': (c_char_p, []),
@@ -87,6 +98,9 @@ _SIGNATURES = {
     'dtb_optim_rows_apply_lr': (c_int, [P, P, P, P, P, P, P, P, P, c_int, P, _OPP, c_int, c_int, c_int, P]),
     'dtb_optim_dense_reg_lr': (c_int, [P, P, P, P, P, c_int64, _OPP, P, c_int, P, c_int, c_float, c_float, P, c_double,
                                        P]),
+    'dtb_metrics_state_bytes': (c_size_t, [_MPP]),
+    'dtb_metrics_reset': (c_int, [P, _MPP, P]),
+    'dtb_metrics_update': (c_int, [P, P, P, P, c_int, _MPP, P]),
     'dtb_grad_rows_pack':(c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),

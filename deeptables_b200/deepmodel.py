@@ -24,7 +24,8 @@ from typing import Union
 import numpy as np
 import torch
 
-from . import consts, deepnets, dp, engine as E, layers as L, optimizers as O, regularizers as R, schedules as S
+from . import consts, deepnets, dp, engine as E, layers as L, metrics as M, optimizers as O, regularizers as R, \
+    schedules as S
 from ._native import ptr, check, stream_ptr
 from . import _native as N
 
@@ -316,6 +317,10 @@ class DeepModel:
         self._opt = None                   # optimizers.OptimizerSpec resolved from ModelConfig.optimizer
         self._opt_native = None            # its dtb_optim_params (SGD / RMSprop / Adagrad)
         self._emb_reg = None               # regularizers.RegSpec of ModelConfig.embeddings_regularizer
+        self._metric_fns = None            # ModelConfig.metrics: functions of a whole epoch's predictions (_resolve_metrics)
+        self._metric_keys = ()             # every metric's history key, in ModelConfig.metrics order
+        self._metrics_train = None         # engine.MetricsState of the streaming metrics (metrics.py): training batches
+        self._metrics_eval = None          # ... and validation / evaluate batches
         self._graphs = {}
         self._graph_failed = False
         if model_file is not None:
@@ -341,6 +346,12 @@ class DeepModel:
             self._focal = (cfg.loss.gamma, cfg.loss.alpha)
         elif cfg.loss != 'auto':
             raise NotImplementedError("loss must be 'auto' or one of layers.BinaryFocalLoss / CategoricalFocalLoss")
+        self._metric_fns, specs, self._metric_keys = _plan_metrics(cfg.metrics, self.task, self.num_classes)
+        self._metrics_train = self._metrics_eval = None
+        if specs:
+            plan = M.Plan(specs, self._output_dim())
+            self._metrics_train = E.MetricsState(plan, self.device)
+            self._metrics_eval = E.MetricsState(plan, self.device)
         R.reject_activity(cfg.embeddings_activity_regularizer, 'embeddings_activity_regularizer')
         self._emb_reg = R.resolve(cfg.embeddings_regularizer, 'embeddings_regularizer')
         if self.task not in consts.ALL_TASKS:
@@ -378,6 +389,7 @@ class DeepModel:
             self.task, 'binary_crossentropy' if self.num_classes == 2 else 'categorical_crossentropy')
         if self._focal is not None:
             self.model_desc.loss = 'focal_loss'
+        self.model_desc.metrics = [str(spec) for spec in specs]
         # dry run on two rows materialises every weight (define-by-run build)
         cat = torch.zeros(2, self.n_fields, dtype=torch.int32, device=self.device) if self.n_fields else None
         cont = torch.zeros(2, self.n_cont, dtype=torch.float32, device=self.device) if self.n_cont else None
@@ -592,6 +604,8 @@ class DeepModel:
         z = self._forward(cat, cont, training=True)
         scope.seed_sites = scope._seed_counter - seeds_before
         prob, dz = E.loss_forward_backward(z, y, self.task, sample_weight, True, self._loss_acc, focal=self._focal)
+        if self._metrics_train is not None:
+            self._metrics_train.update(prob, y)      # unweighted, as Keras's `metrics=` are
         dp.scale_for_mean(dz)
         z.backward(dz)
         step = self._step + 1
@@ -920,7 +934,7 @@ class DeepModel:
         self.stop_training = False
         for cb in callbacks:
             _call(cb, 'on_train_begin', None)
-        metric_fns = _resolve_metrics(self.config.metrics, self.task)
+        metric_fns = self._metric_fns
         # train batches drop the remainder only when there is at least one full batch
         # (reference dataset_generator.py:70)
         drop_remainder = n >= batch_size
@@ -931,6 +945,8 @@ class DeepModel:
             pdev = 'cpu' if on_host else self.device
             perm = torch.randperm(n, device=pdev) if shuffle else torch.arange(n, device=pdev)
             self._loss_acc.zero_()
+            if self._metrics_train is not None:
+                self._metrics_train.reset()
             seen = 0
             probs, targets = [], []
 
@@ -959,27 +975,31 @@ class DeepModel:
                     probs.append(p)
                     targets.append(by)
             logs = {'loss': float(self._loss_acc.item()) / max(seen, 1)}
-            if metric_fns:
-                pp, tt = torch.cat(probs), torch.cat(targets)
-                for name, fn in metric_fns.items():
-                    logs[name] = fn(tt, pp)
+            logs.update(self._metric_logs(metric_fns, probs, targets, self._metrics_train, all_ranks=True))
             if self.table is not None:
                 self.table.check_status()
             self.sync_replica_buffers()          # before validation / callbacks snapshot or score the model
             if (epoch + 1) % validation_freq == 0 and n_val > 0:
-                vlogs = self._evaluate_tensors(vcat, vcont, vy, batch_size, validation_steps, metric_fns)
+                vlogs = self._evaluate_tensors(vcat, vcont, vy, batch_size, validation_steps, metric_fns,
+                                               all_ranks=True)
                 if self._dist and vlogs:
-                    # same validation logs on every rank (mean over the ranks' shards), so callbacks such as
-                    # EarlyStopping(restore_best_weights) take identical decisions and the replicas stay identical
-                    keys = sorted(vlogs)
+                    # same validation logs on every rank, so callbacks such as EarlyStopping(restore_best_weights)
+                    # take identical decisions and the replicas stay identical: the loss and the epoch functions are
+                    # averaged over the ranks' shards; the streaming metrics already are those of all shards together
+                    keys = sorted(k for k in vlogs if k == 'loss' or k in metric_fns)
                     vt = torch.tensor([float(vlogs[k]) for k in keys], dtype=torch.float64, device=self.device)
                     torch.distributed.all_reduce(vt)
-                    vlogs = dict(zip(keys, (vt / self.world_size).tolist()))
+                    vlogs.update(zip(keys, (vt / self.world_size).tolist()))
                 logs.update({f'val_{k}': v for k, v in vlogs.items()})
             if verbose:
-                msg = ' - '.join(f'{k}: {v:.4f}' for k, v in logs.items())
+                msg = ' - '.join(f'{k}: ' + (f'{v:.4f}' if isinstance(v, float) else str(v)) for k, v in logs.items())
                 print(f'Epoch {epoch + 1}/{epochs} - {steps_per_epoch} steps - {msg}')
             for cb in callbacks:
+                monitored = logs.get(getattr(cb, 'monitor', None))
+                if isinstance(monitored, list):
+                    raise ValueError(f'{type(cb).__name__} monitors {cb.monitor!r}, which has one value per threshold or '
+                                     f'class ({monitored}); monitor a metric with a single value, such as F1Score with '
+                                     f"average='macro' or Precision with one threshold")
                 _call(cb, 'on_epoch_end', epoch, logs)
             self._agree_learning_rate()
             # recorded after the callbacks, as Keras's History (the last callback) does: keys they add, such as
@@ -1015,11 +1035,37 @@ class DeepModel:
         elif ov is not None:
             self._rates.clear_override(self._step)
 
-    def _evaluate_tensors(self, cat, cont, y, batch_size, steps, metric_fns):
+    def _metric_logs(self, metric_fns, probs, targets, streaming, all_ranks=False):
+        """The metric part of an epoch's or an evaluation's logs, keyed and ordered as ModelConfig.metrics: the epoch
+        functions on the collected batches, the streaming metrics from one read of their state.  ``all_ranks``: under
+        data parallel the streaming state of every rank is added first (counters exactly, float64 sums in rank order),
+        so every rank gets the metric of all shards together; every rank must then make this call."""
+        values = {}
+        if metric_fns:
+            pp, tt = torch.cat(probs), torch.cat(targets)
+            for name, fn in metric_fns.items():
+                values[name] = fn(tt, pp)
+        if streaming is not None:
+            if all_ranks and self._dist:
+                c = streaming.plan.counters
+                counters = streaming.state[c:].clone()
+                torch.distributed.all_reduce(counters)
+                sums = torch.empty(self.world_size, c, dtype=torch.int64, device=self.device)
+                torch.distributed.all_gather_into_tensor(sums, streaming.state[:c])
+                state = streaming.plan.merge(counters.cpu().numpy(), sums.cpu().numpy().view('float64'))
+            else:
+                state = streaming.read()
+            values.update(streaming.plan.finish(state))
+        return OrderedDict((k, values[k]) for k in self._metric_keys if k in values)
+
+    def _evaluate_tensors(self, cat, cont, y, batch_size, steps, metric_fns, all_ranks=False):
         n = y.shape[0]
         loss_acc = torch.zeros(1, dtype=torch.float64, device=self.device)
         probs, targets = [], []
         seen = 0
+        streaming = self._metrics_eval
+        if streaming is not None:
+            streaming.reset()
         for step in range(steps):
             lo = step * batch_size
             if lo >= n:
@@ -1032,15 +1078,27 @@ class DeepModel:
             with torch.no_grad():
                 z = self._forward(bc, bx, training=False)
                 p, _ = E.loss_forward_backward(z, by, self.task, None, False, loss_acc, focal=self._focal)
-            probs.append(p)
-            targets.append(by)
+            if streaming is not None:
+                streaming.update(p, by)
+            if metric_fns:
+                probs.append(p)
+                targets.append(by)
             seen += by.shape[0]
         self._reg_loss(loss_acc, seen)          # Keras's compute_loss adds model.losses in evaluation too
         logs = {'loss': float(loss_acc.item()) / max(seen, 1)}
-        pp, tt = torch.cat(probs), torch.cat(targets)
-        for name, fn in metric_fns.items():
-            logs[name] = fn(tt, pp)
+        logs.update(self._metric_logs(metric_fns, probs, targets, streaming, all_ranks))
         return logs
+
+    def streaming_scores(self, metrics, y, proba):
+        """Streaming metrics (metrics.py: objects or names) of labels ``y``, as fit takes them, and predictions ``proba``
+        as predict returns them: history key -> value."""
+        if self.model is None:
+            raise RuntimeError('model is not built: call fit() or load a model first')
+        specs = [M.resolve(m, self.task, self.num_classes) for m in metrics]
+        state = E.MetricsState(M.Plan(specs, self._output_dim()), self.device)
+        p = torch.as_tensor(np.ascontiguousarray(proba, dtype=np.float32)).reshape(len(proba), -1).to(self.device)
+        state.update(p, self._to_device_labels(y))
+        return state.plan.finish(state.read())
 
     def predict(self, X, batch_size=128, verbose=0):
         return self.__predict(X, batch_size=batch_size, verbose=verbose)
@@ -1096,7 +1154,7 @@ class DeepModel:
         cat, cont = self._to_device_inputs(X_test)
         y = self._to_device_labels(y_test)
         steps = math.ceil(_length(X_test) / batch_size)
-        logs = self._evaluate_tensors(cat, cont, y, batch_size, steps, _resolve_metrics(self.config.metrics, self.task))
+        logs = self._evaluate_tensors(cat, cont, y, batch_size, steps, self._metric_fns)
         if return_dict:
             return IgnoreCaseDict(logs)
         return list(logs.values())
@@ -1478,6 +1536,10 @@ def _auc(y_true, y_prob):
     return (s - n_pos * (n_pos + 1) / 2.0) / (n_pos * n_neg)
 
 
+_EPOCH_METRIC_NAMES = ('auc', 'accuracy', 'acc', 'mse', 'mean_squared_error', 'rmse', 'rootmeansquarederror',
+                       'root_mean_squared_error', 'mae', 'mean_absolute_error')     # the strings _resolve_metrics knows
+
+
 def _resolve_metrics(metrics, task):
     fns = OrderedDict()
     for m in (metrics or []):
@@ -1503,6 +1565,30 @@ def _resolve_metrics(metrics, task):
     return fns
 
 
+def _plan_metrics(metrics, task, num_classes):
+    """ModelConfig.metrics -> (epoch functions by key, streaming MetricSpecs, every key in the order given).
+
+    An object of one of metrics.py's class names with get_config() is a streaming metric, whatever its name.  The
+    strings and plain functions _resolve_metrics knows keep the function, key and value they have there.  The other
+    names metrics.py knows are streaming metrics.  Anything else raises NotImplementedError, and two entries whose
+    keys differ at most in case (History is case-insensitive) raise ValueError."""
+    fns, specs, keys = OrderedDict(), [], []
+    for m in (metrics or []):
+        if M.is_metric_object(m):
+            specs.append(M.resolve(m, task, num_classes))
+            key = specs[-1].key
+        elif isinstance(m, str) and m.lower() not in _EPOCH_METRIC_NAMES and M.is_metric_name(m):
+            specs.append(M.resolve(m, task, num_classes))
+            key = m
+        else:
+            (key, fn), = _resolve_metrics([m], task).items()
+            fns[key] = fn
+        if key.lower() in (k.lower() for k in keys):
+            raise ValueError(f'ModelConfig.metrics has two entries named {key!r}: give one of them another name=')
+        keys.append(key)
+    return fns, specs, tuple(keys)
+
+
 class ModelDesc:
     """Human-readable description of the built model (reference deepmodel.py:460-532)."""
 
@@ -1511,6 +1597,7 @@ class ModelDesc:
         self.embeddings = self.dense = self.concat_embed_dense = None
         self.stacking = self.output = self.loss = self.optimizer = None
         self.regularizers = []             # 'weight name: regularizer' of the regularized Dense kernels
+        self.metrics = []                  # the streaming metrics (metrics.MetricSpec) as text
 
     def add_input(self, name, num_columns):
         self.inputs.append(f'{name}: ({num_columns})')
@@ -1546,6 +1633,8 @@ class ModelDesc:
                 ('concat_embed_dense', self.concat_embed_dense), ('nets', f'{self.nets}\n{self.nets_desc()}'),
                 ('stacking_op', self.stacking), ('output', self.output), ('loss', self.loss),
                 ('optimizer', self.optimizer_info())]
+        if self.metrics:
+            rows.append(('metrics', '\n'.join(self.metrics)))
         if self.regularizers:
             rows.insert(5, ('regularizers', '\n'.join(self.regularizers)))
         body = f'\n{bar}\n'.join(f'{k}: {v}' for k, v in rows)

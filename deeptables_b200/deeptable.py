@@ -31,8 +31,8 @@ class EarlyStopping:
         self.verbose, self.restore_best_weights = verbose, restore_best_weights
         if mode == 'auto':
             lower = monitor.lower()
-            mode = 'max' if any(k in lower for k in ('acc', 'auc', 'fmeasure', 'f1', 'precision', 'recall')) \
-                else 'min'
+            mode = 'max' if any(k in lower for k in ('acc', 'auc', 'fmeasure', 'f1', 'precision', 'recall', 'r2', 'fbeta',
+                                                     'true_positives', 'true_negatives')) else 'min'
         self.mode = mode
         self.model = None
 
@@ -206,6 +206,16 @@ class DefaultPreprocessor:
         return list(self._cont_names)
 
 
+_OOF_SKLEARN_NAMES = ('auc', 'roc_auc', 'accuracy', 'acc', 'f1', 'f1_score', 'logloss', 'log_loss', 'mse',
+                      'mean_squared_error', 'rmse', 'mae', 'mean_absolute_error', 'r2', 'r2_score')
+
+
+def _is_streaming_metric(m):
+    """An ``oof_metrics`` entry that metrics.py computes: its objects, and its names that _calc_scores does not take."""
+    from . import metrics as M
+    return M.is_metric_object(m) or (isinstance(m, str) and m.lower() not in _OOF_SKLEARN_NAMES and M.is_metric_name(m))
+
+
 def _calc_scores(y_true, y_pred, y_proba, task, metrics, pos_label, classes):
     """Scores of one fold for ``oof_metrics`` (the reference delegates to hypernets' calc_score): metric name -> value."""
     from sklearn import metrics as M
@@ -357,7 +367,12 @@ class DeepTable:
                 y_true = self.preprocessor.inverse_transform_y(y[valid_idx])
                 y_proba = self._fix_softmax_proba(fold_oof.copy()) if self.task == consts.TASK_BINARY else fold_oof.copy()
                 y_pred = self.proba2predict(y_proba, encode_to_label=True)
-                oof_scores.append(_calc_scores(y_true, y_pred, y_proba, self.task, oof_metrics, self.pos_label, self.classes_))
+                streaming = [m for m in oof_metrics if _is_streaming_metric(m)]
+                scores = _calc_scores(y_true, y_pred, y_proba, self.task,
+                                      [m for m in oof_metrics if not _is_streaming_metric(m)], self.pos_label, self.classes_)
+                if streaming:           # the names and objects of metrics.py, on the fold's encoded labels and raw output
+                    scores.update(model.streaming_scores(streaming, y[valid_idx], fold_oof))
+                oof_scores.append(scores)
             name = f'{"+".join(self.nets)}-kfold-{n_fold + 1}'
             model.save(f'{self.output_path}{"_".join(self.nets)}-kfold-{n_fold + 1}.npz')
             self.__modelset[name] = (model, history.history)

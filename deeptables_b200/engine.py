@@ -849,6 +849,42 @@ def loss_forward_backward(z, y_true, task, sample_weight=None, want_grad=True, l
     return prob, dz
 
 
+class MetricsState:
+    """Device state of one model's streaming metrics (metrics.Plan): the counters and sums ``dtb_metrics_update`` adds
+    each batch to, the threshold lists it reads, and the ``dtb_metric_plan`` that describes both."""
+
+    def __init__(self, plan, device):
+        self.plan = plan
+        n = N.MetricPlan(cols=plan.cols, n_lists=len(plan.lists), sums=plan.sums, argmax=int(plan.argmax),
+                         top_k=plan.top_k)
+        for i, lst in enumerate(plan.lists):
+            n.list_len[i], n.list_off[i] = len(lst), plan.list_off[i]
+        self.native = n
+        words = N.lib.dtb_metrics_state_bytes(n) // 8
+        if words != plan.words:
+            raise RuntimeError(f'metric state layout mismatch: library {words} words, metrics.Plan {plan.words}')
+        self.state = torch.zeros(words, dtype=torch.int64, device=device)
+        self.thresholds = torch.as_tensor(plan.thresholds()).to(device)
+
+    def reset(self):
+        check(N.lib.dtb_metrics_reset(ptr(self.state), self.native, stream_ptr()), 'metrics_reset')
+
+    def update(self, prob, y_true):
+        """Add one batch: ``prob`` and ``y_true`` float32 [rows, plan.cols] in device memory."""
+        prob, y_true = _f32(prob), _f32(y_true)
+        if prob.dim() != 2 or prob.shape[1] != self.plan.cols or y_true.numel() != prob.numel():
+            raise ValueError(f'metrics: expected [rows, {self.plan.cols}] predictions and labels, got '
+                             f'{tuple(prob.shape)} and {tuple(y_true.shape)}')
+        if prob.shape[0] == 0:
+            return
+        check(N.lib.dtb_metrics_update(ptr(prob), ptr(y_true), ptr(self.state), ptr(self.thresholds), prob.shape[0],
+                                       self.native, stream_ptr()), 'metrics_update')
+
+    def read(self):
+        """The state as a host uint64 array (one device-to-host copy)."""
+        return self.state.cpu().numpy().view('uint64')
+
+
 def adam_alpha(step, lr=1e-3, b1=ADAM_B1, b2=ADAM_B2):
     """lr * sqrt(1 - b2^t) / (1 - b1^t)  (keras Adam.update_step)."""
     return lr * math.sqrt(1.0 - b2 ** step) / (1.0 - b1 ** step)

@@ -268,6 +268,50 @@ int dtb_optim_dense_reg_lr(float* p, float* g, float* s0, float* s1, float* s2, 
                            const float* lr_table, int step, const int32_t* step_dev, int zero_grad, float l1, float l2,
                            double* loss_acc, double loss_scale, void* stream);
 
+/* ---- streaming metrics (keras.metrics accumulators; deepmodel.py:319-346 passes ModelConfig.metrics to compile) --- */
+/* One device buffer `state` of 8-byte words holds every configured metric of a model; one dtb_metrics_update per
+ * batch adds the batch to all of them.  Layout, with C = plan->cols:
+ *   words [0, 8)              float64 sums over rows of the row means (over the C columns) of DTB_METRIC_SUM_* in bit
+ *                             order: (p-y)^2, |p-y|, 100|p-y|/max(|y|,1e-7), (log(max(p,1e-7)+1)-log(max(y,1e-7)+1))^2,
+ *                             log cosh(p-y), binary and categorical cross-entropy on probabilities; word 7 unused
+ *   words [8, 8+3C)           float64 per column: sum y, sum y^2, sum (y-p)^2                 (DTB_METRIC_SUM_R2)
+ *   counters from word 8+3C   uint64: [0] rows; [1] rows whose first arg-max of p is the first arg-max of y; [2] rows
+ *                             whose p at the first arg-max of y is finite and exceeded by fewer than top_k others;
+ *                             [3+kC+c], k = 0,1,2: TP, FP, FN of column c with the prediction "p_c is the row maximum
+ *                             and |p_c| > 1e-9" (keras FBetaScore without a threshold); then for every threshold list
+ *                             l in order a histogram [C][2][list_len[l]+1]: bucket j of (column c, label y_c != 0)
+ *                             counts the elements with exactly j thresholds strictly below p (keras tests p > t), so
+ *                             TP(t_i) is the sum of the label-1 buckets above i.  A NaN p is above no threshold.
+ * Each list is ascending float32 at thresholds_dev[list_off[l] ..]; all lists together hold at most
+ * DTB_METRIC_MAX_THRESHOLDS values.  The counters are integers added with atomics: the same batches give the same
+ * bits whatever the block scheduling, eagerly or replayed from a CUDA graph.  The float64 sums are warp-reduced and
+ * added with atomicAdd(double), as the loss sum of dtb_loss_fwd_bwd is: their last bits depend on the order.
+ * Arg-max counters are kept only when plan->argmax is set, sums only for the bits of plan->sums.  The update reads
+ * device memory and the plan only (no per-step host scalar): it can be captured in a CUDA graph. */
+#define DTB_METRIC_MAX_LISTS 8
+#define DTB_METRIC_MAX_THRESHOLDS 2048
+#define DTB_METRIC_SUM_SE 1
+#define DTB_METRIC_SUM_AE 2
+#define DTB_METRIC_SUM_APE 4
+#define DTB_METRIC_SUM_SLE 8
+#define DTB_METRIC_SUM_LOGCOSH 16
+#define DTB_METRIC_SUM_BCE 32
+#define DTB_METRIC_SUM_CCE 64
+#define DTB_METRIC_SUM_R2 128
+typedef struct dtb_metric_plan {
+  int cols;                            /* columns of prob / y_true */
+  int n_lists;                         /* threshold lists, <= DTB_METRIC_MAX_LISTS */
+  int list_len[DTB_METRIC_MAX_LISTS];  /* thresholds per list, >= 1 */
+  int list_off[DTB_METRIC_MAX_LISTS];  /* first threshold of the list in thresholds_dev */
+  int sums;                            /* DTB_METRIC_SUM_* bits */
+  int argmax;                          /* keep the arg-max counters [1], [2] and the per-column TP / FP / FN */
+  int top_k;                           /* k of counter [2], >= 1 when argmax is set */
+} dtb_metric_plan;
+size_t dtb_metrics_state_bytes(const dtb_metric_plan* plan);
+int dtb_metrics_reset(void* state, const dtb_metric_plan* plan, void* stream);
+int dtb_metrics_update(const float* prob, const float* y_true, void* state, const float* thresholds_dev, int rows,
+                       const dtb_metric_plan* plan, void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
