@@ -45,6 +45,14 @@ class MetricPlan(ctypes.Structure):
 
 _MPP = POINTER(MetricPlan)
 
+
+class LossParams(ctypes.Structure):
+    """``dtb_loss_params`` (host memory, read at call time): the loss ``dtb_keras_loss_fwd_bwd`` computes."""
+    _fields_ = [('loss', c_int), ('delta', c_float), ('label_smoothing', c_float), ('scratch', c_void_p)]
+
+
+_LPP = POINTER(LossParams)
+
 _SIGNATURES = {
     'dtb_version': (c_int, []),
     'dtb_last_error': (c_char_p, []),
@@ -71,6 +79,7 @@ _SIGNATURES = {
     'dtb_seed_advance': (c_int, [P, c_int, P]),
     'dtb_loss_fwd_bwd': (c_int, [P, P, P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_focal_loss_fwd_bwd': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_float, c_float, P]),
+    'dtb_keras_loss_fwd_bwd': (c_int, [P, P, P, P, P, P, c_int, c_int, c_int, _LPP, P]),
     'dtb_adam_dense': (c_int, [P, P, P, P, c_int64, c_float, c_double, c_double, c_float, c_int, P]),
     'dtb_adam_rows_catchup': (c_int, [P, P, P, P, P, P, P, c_int, c_double, c_double, c_float,
                                       c_int, c_int, c_int, P]),

@@ -1,10 +1,13 @@
 // BatchNormalization, Dense, task losses and the dense Adam step.
 //   BN     : keras BatchNormalization(axis=-1)  (deepmodel.py:359, layers.py:152, deepnets.py:422)
 //   Dense  : keras Dense                        (deepnets.py:415-424, deepmodel.py:292,455)
-//   losses : sigmoid+BCE / MSE / softmax+CCE    (deepmodel.py:319-346,436-457)
+//   losses : sigmoid+BCE / MSE / softmax+CCE    (deepmodel.py:319-346,436-457), the focal losses and
+//            Keras 3's MAE, MAPE, MSLE, Huber, LogCosh, Poisson, the hinge losses, KL divergence and
+//            label-smoothed BCE / CCE (ModelConfig.loss, losses.py)
 //   Adam   : keras.optimizers.Adam.update_step  (deepmodel.py:321-322)
 // The Dense GEMMs are plain fp32 library GEMMs (cuBLAS Sgemm); everything around them (bias,
 // activation, narrow logit layers, reductions) is hand-written.  All of it is HBM-bound streaming.
+#include <cfloat>
 #include "dtb_common.cuh"
 #include "dense_tc.h"
 
@@ -357,6 +360,192 @@ __global__ void focal_loss_kernel(const float* __restrict__ z, const float* __re
 }
 
 // ------------------------------------------------------------------------------------------
+// Keras 3 losses passed as ModelConfig.loss (losses.py), on the task output p of the pre-activation z:
+// sigmoid (task 0), identity (task 1), softmax (task 2).  Per row: the loss l and, with dz, dz = w / rows * dl/dz,
+// the derivative of the float32 expressions below under TensorFlow's conventions (clip passes the gradient on
+// [lo, hi], maximum(a, b) to a where a >= b, abs'(0) = 0, a max over columns splits it among ties, where() to the
+// branch taken).  Three passes over a row, all by the thread that owns it: the output (and CategoricalHinge's row
+// statistics), the loss terms with g = d(term)/dp, then -- softmax or CategoricalCrossentropy only -- the chain
+// through the renormalisation q = p / sum p and the softmax Jacobian, dz_k = p_k (h_k - sum_c h_c p_c).
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ float sign_f(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f); }
+
+// *not_binary = 1 when some label is neither 0 nor 1 (keras convert_binary_labels_to_hinge, batch-wide);
+// the caller zeroes it first
+__global__ void hinge_labels_kernel(const float* __restrict__ y, int64_t n, int* __restrict__ not_binary) {
+  bool other = false;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float v = y[i];
+    other |= !(v == 0.f || v == 1.f);
+  }
+  if (__syncthreads_or(other) && threadIdx.x == 0) *not_binary = 1;
+}
+
+__global__ void keras_loss_kernel(const float* __restrict__ z, const float* __restrict__ y,
+                                  const float* __restrict__ sw, float* __restrict__ prob, float* __restrict__ dz,
+                                  double* __restrict__ loss_sum, int rows, int cols, int task, int loss, float delta,
+                                  float smoothing, const int* __restrict__ not_binary) {
+  const float eps = 1e-7f;
+  const bool to_pm1 = not_binary != nullptr && *not_binary == 0;     // hinge labels 0 / 1 -> -1 / 1
+  const bool cce = loss == DTB_LOSS_CATEGORICAL_CROSSENTROPY;
+  const bool summed = cce || loss == DTB_LOSS_KL_DIVERGENCE || loss == DTB_LOSS_CATEGORICAL_HINGE;   // else mean_c
+  const bool late = task == 2 || cce;                                // dz needs a third pass over the row
+  const float inv_c = 1.f / (float)cols;
+  const float y_off = loss == DTB_LOSS_BINARY_CROSSENTROPY ? 0.5f * smoothing : smoothing * inv_c;
+  double local = 0.0;
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x) {
+    const float w = sw ? sw[r] : 1.f;
+    const float* zr = z + (int64_t)r * cols;
+    const float* yr = y + (int64_t)r * cols;
+    float* pr = prob + (int64_t)r * cols;
+    float* dr = dz ? dz + (int64_t)r * cols : nullptr;
+    // pass 1: the task output; the row sum (renormalisation) and CategoricalHinge's pos / neg / ties
+    float mx = -INFINITY, den = 0.f;
+    if (task == 2) {
+      for (int c = 0; c < cols; ++c) mx = fmaxf(mx, zr[c]);
+      for (int c = 0; c < cols; ++c) den += expf(zr[c] - mx);
+    }
+    float s = 0.f, pos = 0.f, neg = -INFINITY;
+    int ties = 0;
+    for (int c = 0; c < cols; ++c) {
+      const float p = task == 0 ? 1.f / (1.f + expf(-zr[c])) : (task == 1 ? zr[c] : expf(zr[c] - mx) / den);
+      pr[c] = p;
+      s += p;
+      if (loss == DTB_LOSS_CATEGORICAL_HINGE) {
+        const float t = (1.f - yr[c]) * p;
+        pos += yr[c] * p;
+        if (t > neg) {
+          neg = t;
+          ties = 1;
+        } else if (t == neg) {
+          ++ties;
+        }
+      }
+    }
+    const float margin = neg - pos + 1.f;                         // CategoricalHinge
+    const bool ch_active = margin >= 0.f;
+    // pass 2: loss terms and g = d(term)/dp (CategoricalCrossentropy: d/dq); g*p and g*q summed for pass 3
+    float row = 0.f, gp = 0.f, gq = 0.f;
+    const float scale = w / (float)rows;
+    for (int c = 0; c < cols; ++c) {
+      const float p = pr[c];
+      const float yc = yr[c];
+      float v = 0.f, g = 0.f;
+      switch (loss) {
+        case DTB_LOSS_MEAN_SQUARED_ERROR: {
+          const float e = p - yc;
+          v = e * e;
+          g = 2.f * e;
+          break;
+        }
+        case DTB_LOSS_MEAN_ABSOLUTE_ERROR:
+          v = fabsf(yc - p);
+          g = -sign_f(yc - p);
+          break;
+        case DTB_LOSS_MEAN_ABSOLUTE_PERCENTAGE_ERROR: {
+          const float d = fmaxf(fabsf(yc), eps);
+          const float q = (yc - p) / d;
+          v = 100.f * fabsf(q);
+          g = -100.f * sign_f(q) / d;
+          break;
+        }
+        case DTB_LOSS_MEAN_SQUARED_LOGARITHMIC_ERROR: {
+          const float pm = fmaxf(p, eps);
+          const float e = logf(pm + 1.f) - logf(fmaxf(yc, eps) + 1.f);
+          v = e * e;
+          g = p >= eps ? 2.f * e / (pm + 1.f) : 0.f;
+          break;
+        }
+        case DTB_LOSS_HUBER: {
+          const float e = p - yc, ae = fabsf(e);
+          if (ae <= delta) {
+            v = 0.5f * (e * e);
+            g = e;
+          } else {
+            v = delta * ae - 0.5f * (delta * delta);
+            g = delta * sign_f(e);
+          }
+          break;
+        }
+        case DTB_LOSS_LOG_COSH: {
+          const float e = p - yc, a = -2.f * e;
+          const float softplus = a > 0.f ? a + log1pf(expf(-a)) : log1pf(expf(a));
+          v = e + softplus - 0.69314718f;
+          g = 1.f - 2.f / (1.f + expf(-a));                       // 1 - 2 sigmoid(-2e)
+          break;
+        }
+        case DTB_LOSS_POISSON:
+          v = p - yc * logf(p + eps);
+          g = 1.f - yc / (p + eps);
+          break;
+        case DTB_LOSS_HINGE:
+        case DTB_LOSS_SQUARED_HINGE: {
+          const float yy = to_pm1 ? 2.f * yc - 1.f : yc;
+          const float m = 1.f - yy * p;
+          const float h = fmaxf(m, 0.f);
+          const bool sq = loss == DTB_LOSS_SQUARED_HINGE;
+          v = sq ? h * h : h;
+          g = m >= 0.f ? (sq ? -2.f * h * yy : -yy) : 0.f;
+          break;
+        }
+        case DTB_LOSS_CATEGORICAL_HINGE:
+          g = ch_active ? (((1.f - yc) * p == neg ? (1.f - yc) / (float)ties : 0.f) - yc) : 0.f;
+          break;
+        case DTB_LOSS_KL_DIVERGENCE: {
+          const float yh = fminf(fmaxf(yc, eps), 1.f), ph = fminf(fmaxf(p, eps), 1.f);
+          v = yh * logf(yh / ph);
+          g = (p >= eps && p <= 1.f) ? -yh / ph : 0.f;
+          break;
+        }
+        case DTB_LOSS_BINARY_CROSSENTROPY: {
+          const float ys = yc * (1.f - smoothing) + y_off;
+          const float pc = fminf(fmaxf(p, eps), 1.f - eps);
+          v = -(ys * logf(pc) + (1.f - ys) * logf(1.f - pc));
+          g = (p >= eps && p <= 1.f - eps) ? (1.f - ys) / (1.f - pc) - ys / pc : 0.f;
+          break;
+        }
+        default: {                                                // DTB_LOSS_CATEGORICAL_CROSSENTROPY
+          const float ys = yc * (1.f - smoothing) + y_off;
+          const float q = p / s;
+          const float qc = fminf(fmaxf(q, eps), 1.f - eps);
+          v = -ys * logf(qc);
+          g = (q >= eps && q <= 1.f - eps) ? -ys / qc : 0.f;
+          gq += g * q;
+          break;
+        }
+      }
+      row += v;
+      if (!summed) g *= inv_c;
+      if (dr) {
+        if (late) {
+          dr[c] = g;
+          gp += g * p;
+        } else {
+          dr[c] = (task == 0 ? g * (p * (1.f - p)) : g) * scale;
+        }
+      }
+    }
+    if (loss == DTB_LOSS_CATEGORICAL_HINGE) row = fmaxf(margin, 0.f);
+    else if (!summed) row /= (float)cols;
+    // pass 3: h = dl/dp through the renormalisation (h_k = (g_k - sum g q) / s), then the activation
+    if (dr && late) {
+      const float inv_s = cce ? 1.f / s : 1.f;
+      const float hp = cce ? (gp - gq * s) * inv_s : gp;           // sum_c h_c p_c
+      for (int c = 0; c < cols; ++c) {
+        const float p = pr[c];
+        float h = cce ? (dr[c] - gq) * inv_s : dr[c];
+        if (task == 0) h *= p * (1.f - p);
+        else if (task == 2) h = p * (h - hp);
+        dr[c] = h * scale;
+      }
+    }
+    local += (double)(row * w);
+  }
+  local = warp_sum(local);
+  if (loss_sum && (threadIdx.x & 31) == 0 && local != 0.0) atomicAdd(loss_sum, local);
+}
+
+// ------------------------------------------------------------------------------------------
 // Dropout (keras Dropout / SpatialDropout1D on (B,1,D) field embeddings == element-wise): counter-based
 // mask, so forward and backward regenerate the same bits from (seed, element index); nothing is stored.
 // ------------------------------------------------------------------------------------------
@@ -571,6 +760,33 @@ int dtb_focal_loss_fwd_bwd(const float* z, const float* y_true, float* prob, flo
   const int cap = sm_count() * 8;
   if (blocks > cap) blocks = cap;
   focal_loss_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(z, y_true, prob, dz, loss_sum, rows, cols, task, gamma, alpha);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
+
+int dtb_keras_loss_fwd_bwd(const float* z, const float* y_true, const float* sample_weight, float* prob, float* dz,
+                           double* loss_sum, int rows, int cols, int task, const dtb_loss_params* lp, void* stream) {
+  DTB_CHECK_ARG(z && y_true && prob && lp, "NULL argument");
+  DTB_CHECK_ARG(rows >= 0 && cols > 0 && task >= 0 && task <= 2, "bad shape/task");
+  const int loss = lp->loss;
+  DTB_CHECK_ARG(loss >= DTB_LOSS_MEAN_SQUARED_ERROR && loss <= DTB_LOSS_CATEGORICAL_CROSSENTROPY, "unknown loss code");
+  DTB_CHECK_ARG(loss != DTB_LOSS_HUBER || (lp->delta > 0.f && lp->delta <= FLT_MAX), "Huber delta must be positive and finite");
+  DTB_CHECK_ARG(lp->label_smoothing >= 0.f && lp->label_smoothing <= 1.f, "label_smoothing must be in [0, 1]");
+  const bool hinge = loss == DTB_LOSS_HINGE || loss == DTB_LOSS_SQUARED_HINGE;
+  DTB_CHECK_ARG(!hinge || lp->scratch, "the hinge losses need lp->scratch (one device int)");
+  if (rows == 0) return DTB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (hinge) {
+    const int64_t n = (int64_t)rows * cols;
+    DTB_CUDA_OK(cudaMemsetAsync(lp->scratch, 0, sizeof(int), st));
+    hinge_labels_kernel<<<ew_grid(n), 256, 0, st>>>(y_true, n, lp->scratch);
+    DTB_LAUNCH_OK();
+  }
+  int blocks = ceil_div(rows, 256);
+  const int cap = sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  keras_loss_kernel<<<blocks, 256, 0, st>>>(z, y_true, sample_weight, prob, dz, loss_sum, rows, cols, task, loss,
+                                            lp->delta, lp->label_smoothing, hinge ? lp->scratch : nullptr);
   DTB_LAUNCH_OK();
   return DTB_OK;
 }

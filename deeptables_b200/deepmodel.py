@@ -5,7 +5,7 @@ Same constructor and public methods (fit / predict / evaluate / apply / save / r
 inputs -> MultiColumnEmbedding -> flatten/concat + BatchNormalization -> net builders -> stacking ->
 ``task_output``), same training contract (Adam(1e-3) + BCE/MSE/CCE when ``optimizer``/``loss`` are
 'auto', reference deepmodel.py:319-346; SGD / RMSprop / Adagrad / Adam at other hyperparameters through
-``optimizers.py``; ``steps_per_epoch`` / ``validation_steps`` arithmetic,
+``optimizers.py``, Keras 3's losses through ``losses.py``; ``steps_per_epoch`` / ``validation_steps`` arithmetic,
 reference deepmodel.py:76-83).  The numerics run in hand-written sm_90a kernels behind the C ABI;
 torch supplies device memory and the autograd tape only.
 
@@ -24,8 +24,8 @@ from typing import Union
 import numpy as np
 import torch
 
-from . import consts, deepnets, dp, engine as E, layers as L, metrics as M, optimizers as O, regularizers as R, \
-    schedules as S
+from . import consts, deepnets, dp, engine as E, layers as L, losses as LS, metrics as M, optimizers as O, \
+    regularizers as R, schedules as S
 from ._native import ptr, check, stream_ptr
 from . import _native as N
 
@@ -312,6 +312,7 @@ class DeepModel:
         self.table = None
         self._loss_acc = None
         self._focal = None                  # (gamma, alpha) when ModelConfig.loss is one of the focal losses
+        self._loss = None                   # losses.LossSpec when ModelConfig.loss is a Keras loss
         self._rates = None                 # _StepRates: the per-step learning rate (Adam: alpha) table in device memory
         self._step_dev = None              # optimiser step counter in device memory (CUDA-graph replay of the train step)
         self._opt = None                   # optimizers.OptimizerSpec resolved from ModelConfig.optimizer
@@ -336,6 +337,7 @@ class DeepModel:
         self._rates = _StepRates(self._opt, self.device)
         slot_inits = None if self._opt.kind == 'adam' else O.slot_inits(self._opt)
         self._focal = None
+        self._loss = None
         if isinstance(cfg.loss, L.CategoricalFocalLoss):
             if self.task != consts.TASK_MULTICLASS:
                 raise ValueError('CategoricalFocalLoss needs a multiclass task')
@@ -344,8 +346,8 @@ class DeepModel:
             if self.task not in (consts.TASK_BINARY, consts.TASK_MULTILABEL):
                 raise ValueError('BinaryFocalLoss needs a binary or multilabel task')
             self._focal = (cfg.loss.gamma, cfg.loss.alpha)
-        elif cfg.loss != 'auto':
-            raise NotImplementedError("loss must be 'auto' or one of layers.BinaryFocalLoss / CategoricalFocalLoss")
+        elif not (isinstance(cfg.loss, str) and cfg.loss == 'auto'):
+            self._loss = LS.resolve(cfg.loss, self.task, self.num_classes)
         self._metric_fns, specs, self._metric_keys = _plan_metrics(cfg.metrics, self.task, self.num_classes)
         self._metrics_train = self._metrics_eval = None
         if specs:
@@ -389,6 +391,8 @@ class DeepModel:
             self.task, 'binary_crossentropy' if self.num_classes == 2 else 'categorical_crossentropy')
         if self._focal is not None:
             self.model_desc.loss = 'focal_loss'
+        elif self._loss is not None:
+            self.model_desc.loss = str(self._loss)
         self.model_desc.metrics = [str(spec) for spec in specs]
         # dry run on two rows materialises every weight (define-by-run build)
         cat = torch.zeros(2, self.n_fields, dtype=torch.int32, device=self.device) if self.n_fields else None
@@ -603,7 +607,8 @@ class DeepModel:
         seeds_before = scope._seed_counter
         z = self._forward(cat, cont, training=True)
         scope.seed_sites = scope._seed_counter - seeds_before
-        prob, dz = E.loss_forward_backward(z, y, self.task, sample_weight, True, self._loss_acc, focal=self._focal)
+        prob, dz = E.loss_forward_backward(z, y, self.task, sample_weight, True, self._loss_acc, focal=self._focal,
+                                           loss=self._loss)
         if self._metrics_train is not None:
             self._metrics_train.update(prob, y)      # unweighted, as Keras's `metrics=` are
         dp.scale_for_mean(dz)
@@ -1077,7 +1082,8 @@ class DeepModel:
                 self._catch_up(bc, self._step)
             with torch.no_grad():
                 z = self._forward(bc, bx, training=False)
-                p, _ = E.loss_forward_backward(z, by, self.task, None, False, loss_acc, focal=self._focal)
+                p, _ = E.loss_forward_backward(z, by, self.task, None, False, loss_acc, focal=self._focal,
+                                               loss=self._loss)
             if streaming is not None:
                 streaming.update(p, by)
             if metric_fns:

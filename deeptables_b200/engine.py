@@ -829,10 +829,12 @@ class AttentionCoreFn(torch.autograd.Function):
 TASK_CODES = {'binary': 0, 'multilabel': 0, 'regression': 1, 'multiclass': 2}
 
 
-def loss_forward_backward(z, y_true, task, sample_weight=None, want_grad=True, loss_acc=None, focal=None):
+def loss_forward_backward(z, y_true, task, sample_weight=None, want_grad=True, loss_acc=None, focal=None, loss=None):
     """task_output activation + loss + dLoss/dz in one launch (deepmodel.py:319-346, 436-457).
     Returns (prob, dz or None); adds the sum of per-row losses to ``loss_acc`` (float64[1]).
-    ``focal`` = (gamma, alpha): the reference's Binary / CategoricalFocalLoss (layers.py:983-1083) instead of BCE / CCE."""
+    ``focal`` = (gamma, alpha): the reference's Binary / CategoricalFocalLoss (layers.py:983-1083) instead of BCE / CCE.
+    ``loss``: a ``losses.LossSpec`` (ModelConfig.loss); where it is the task's own BCE / MSE / CCE the task's kernel
+    runs it, otherwise ``dtb_keras_loss_fwd_bwd`` (the hinge losses add one launch that checks the labels)."""
     z = _f32(z)
     y_true = _f32(y_true).view(z.shape)
     prob = torch.empty_like(z)
@@ -843,6 +845,14 @@ def loss_forward_backward(z, y_true, task, sample_weight=None, want_grad=True, l
             raise NotImplementedError('focal losses take no sample weights')
         check(N.lib.dtb_focal_loss_fwd_bwd(ptr(z), ptr(y_true), ptr(prob), ptr(dz), ptr(loss_acc), rows, cols, TASK_CODES[task],
                                            float(focal[0]), float(focal[1]), stream_ptr()), 'focal_loss_fwd_bwd')
+        return prob, dz
+    if loss is not None and not loss.builtin(task):
+        scratch = torch.empty(1, dtype=torch.int32, device=z.device) if loss.hinge else None
+        lp = N.LossParams(loss=loss.code, delta=loss.delta, label_smoothing=loss.label_smoothing,
+                          scratch=None if scratch is None else scratch.data_ptr())
+        check(N.lib.dtb_keras_loss_fwd_bwd(ptr(z), ptr(y_true), ptr(sample_weight), ptr(prob), ptr(dz), ptr(loss_acc),
+                                           rows, cols, TASK_CODES[task], lp, stream_ptr()),
+              'keras_loss_fwd_bwd')
         return prob, dz
     check(N.lib.dtb_loss_fwd_bwd(ptr(z), ptr(y_true), ptr(sample_weight), ptr(prob), ptr(dz), ptr(loss_acc), rows,
                                  cols, TASK_CODES[task], stream_ptr()), 'loss_fwd_bwd')

@@ -152,6 +152,47 @@ int dtb_focal_loss_fwd_bwd(const float* z, const float* y_true, float* prob, flo
                            double* loss_sum, int rows, int cols, int task, float gamma, float alpha,
                            void* stream);
 
+/* Keras 3 losses passed as ModelConfig.loss (deeptables_b200/losses.py), on the output of `task` (as above:
+ * sigmoid / identity / softmax).  With p the output, y the label row, C = cols and eps = 1e-7, the per-row loss l is
+ *   MEAN_SQUARED_ERROR       mean_c (p - y)^2
+ *   MEAN_ABSOLUTE_ERROR      mean_c |y - p|
+ *   MEAN_ABSOLUTE_PERCENTAGE_ERROR  100 mean_c |(y - p) / max(|y|, eps)|
+ *   MEAN_SQUARED_LOGARITHMIC_ERROR  mean_c (log(max(p, eps) + 1) - log(max(y, eps) + 1))^2
+ *   HUBER                    mean_c (|e| <= delta ? e^2 / 2 : delta |e| - delta^2 / 2),  e = p - y
+ *   LOG_COSH                 mean_c (e + softplus(-2e) - log 2)
+ *   POISSON                  mean_c (p - y log(p + eps))
+ *   HINGE / SQUARED_HINGE    mean_c max(1 - y'p, 0) (squared); y' = 2y - 1 when every label of the batch is 0 or 1
+ *   CATEGORICAL_HINGE        max(max_c((1 - y) p) - sum_c y p + 1, 0)
+ *   KL_DIVERGENCE            sum_c Y log(Y / P),  Y = clip(y, eps, 1), P = clip(p, eps, 1)
+ *   BINARY_CROSSENTROPY      dtb_loss_fwd_bwd's task-0 loss on y (1 - s) + s / 2
+ *   CATEGORICAL_CROSSENTROPY -sum_c y_s log(clip(p / sum p, eps, 1 - eps)),  y_s = y (1 - s) + s / C
+ * s = label_smoothing.  prob, dz, sample_weight and loss_sum as dtb_loss_fwd_bwd: loss_sum += sum_r w_r l_r (float64)
+ * and dz = d(sum_r w_r l_r / rows)/dz under TensorFlow's gradient conventions (clip passes it on [lo, hi],
+ * maximum(a, b) to a where a >= b, abs'(0) = 0, tied maxima share it, Huber at |e| = delta is quadratic);
+ * dz may be NULL.  The hinge losses decide y' on the device (one more launch, into lp->scratch); nothing
+ * synchronises with the host. */
+#define DTB_LOSS_MEAN_SQUARED_ERROR 1
+#define DTB_LOSS_MEAN_ABSOLUTE_ERROR 2
+#define DTB_LOSS_MEAN_ABSOLUTE_PERCENTAGE_ERROR 3
+#define DTB_LOSS_MEAN_SQUARED_LOGARITHMIC_ERROR 4
+#define DTB_LOSS_HUBER 5
+#define DTB_LOSS_LOG_COSH 6
+#define DTB_LOSS_POISSON 7
+#define DTB_LOSS_HINGE 8
+#define DTB_LOSS_SQUARED_HINGE 9
+#define DTB_LOSS_CATEGORICAL_HINGE 10
+#define DTB_LOSS_KL_DIVERGENCE 11
+#define DTB_LOSS_BINARY_CROSSENTROPY 12
+#define DTB_LOSS_CATEGORICAL_CROSSENTROPY 13
+typedef struct dtb_loss_params {  /* host memory, read at call time */
+  int loss;                       /* DTB_LOSS_* */
+  float delta;                    /* HUBER: > 0 and finite */
+  float label_smoothing;          /* s of the two crossentropies, in [0, 1]; 0 for the others */
+  int* scratch;                   /* device int the hinge losses use (NULL for the others) */
+} dtb_loss_params;
+int dtb_keras_loss_fwd_bwd(const float* z, const float* y_true, const float* sample_weight, float* prob, float* dz,
+                           double* loss_sum, int rows, int cols, int task, const dtb_loss_params* lp, void* stream);
+
 /* ---- keras Adam (deepmodel.py:321-322), dense semantics ---------------------------------- */
 /* m += (g-m)(1-b1); v += (g^2-v)(1-b2); p -= m*alpha/(sqrt(v)+eps), alpha computed by caller
  * as lr*sqrt(1-b2^t)/(1-b1^t).  If zero_grad != 0, g is zeroed after use. */
