@@ -110,6 +110,12 @@ _SIGNATURES = {
     'dtb_metrics_state_bytes': (c_size_t, [_MPP]),
     'dtb_metrics_reset': (c_int, [P, _MPP, P]),
     'dtb_metrics_update': (c_int, [P, P, P, P, c_int, _MPP, P]),
+    'dtb_perm_keys': (c_int, [P, c_int64, c_ulonglong, c_int, c_int, P]),
+    'dtb_shuffle_column': (c_int, [P, P, P, c_int64, c_int, c_int, P]),
+    'dtb_importance_scratch_bytes': (c_size_t, [c_int]),
+    'dtb_importance_auc': (c_int, [P, P, P, c_int64, P, P, P]),
+    'dtb_importance_labels': (c_int, [c_int, P, P, c_int64, c_int, c_int, P, P, P]),
+    'dtb_importance_sums': (c_int, [c_int, P, P, P, c_int64, c_int, c_double, P, P, P]),
     'dtb_grad_rows_pack':(c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),

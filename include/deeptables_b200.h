@@ -353,6 +353,37 @@ int dtb_metrics_reset(void* state, const dtb_metric_plan* plan, void* stream);
 int dtb_metrics_update(const float* prob, const float* y_true, void* state, const float* thresholds_dev, int rows,
                        const dtb_metric_plan* plan, void* stream);
 
+/* ---- permutation feature importance (deeptables_b200/importance.py, utils/feature_importance.py) ---------------- */
+/* keys[r] = ((hash(seed, iter, column, r) ^ 2^31) << 32) | r for r < rows < 2^32; sorted as signed 64-bit integers,
+ * their low halves are the permutation of one pass.  seed < 2^32; iter, column >= 0. */
+int dtb_perm_keys(long long* keys, int64_t rows, unsigned long long seed, int iter, int column, void* stream);
+/* dst[b*width + column] = src[perm[b]*width + column] for 4-byte elements, perm[b] the low half of sorted_keys[b];
+ * sorted_keys NULL copies the column back (perm[b] = b).  Other columns of dst are not touched. */
+int dtb_shuffle_column(const void* src, void* dst, const long long* sorted_keys, int64_t rows, int width, int column,
+                       void* stream);
+/* Each scoring call writes one float64 to *out (device memory) and never synchronises with the host.  `scratch` is
+ * device memory of dtb_importance_scratch_bytes(cols) bytes; `prob` is the model output [rows, cols]. */
+#define DTB_IMPORTANCE_AUC 1
+#define DTB_IMPORTANCE_LOG_LOSS 2
+#define DTB_IMPORTANCE_ACCURACY 3
+#define DTB_IMPORTANCE_F1 4          /* binary F1 of class `pos` */
+#define DTB_IMPORTANCE_F1_MACRO 5
+#define DTB_IMPORTANCE_MSE 6
+#define DTB_IMPORTANCE_RMSE 7
+#define DTB_IMPORTANCE_MAE 8
+#define DTB_IMPORTANCE_R2 9
+size_t dtb_importance_scratch_bytes(int cols);
+/* binary ROC AUC from ascending predictions sorted_prob[i] = prob[order[i]] and positive[r] in {0, 1} */
+int dtb_importance_auc(const float* sorted_prob, const long long* order, const int* positive, int64_t rows,
+                       void* scratch, double* out, void* stream);
+/* accuracy / F1 / macro F1 of the predicted class against label[r] (class codes; one column: 0 or 1) */
+int dtb_importance_labels(int metric, const float* prob, const int* label, int64_t rows, int cols, int pos,
+                          void* scratch, double* out, void* stream);
+/* log loss (label[r]: the true column) or, on one column against target[r], MSE / RMSE / MAE / R2 (aux: the sum of
+ * squared deviations of target from its mean) */
+int dtb_importance_sums(int metric, const float* prob, const int* label, const double* target, int64_t rows, int cols,
+                        double aux, void* scratch, double* out, void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
