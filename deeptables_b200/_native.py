@@ -116,6 +116,8 @@ _SIGNATURES = {
     'dtb_importance_auc': (c_int, [P, P, P, c_int64, P, P, P]),
     'dtb_importance_labels': (c_int, [c_int, P, P, c_int64, c_int, c_int, P, P, P]),
     'dtb_importance_sums': (c_int, [c_int, P, P, P, c_int64, c_int, c_double, P, P, P]),
+    'dtb_shap_compose': (c_int, [P, P, P, P, P, c_int, P, P, P, c_int64, c_int, c_int, c_int, P, P, P]),
+    'dtb_shap_means': (c_int, [P, c_int64, c_int, c_int, c_int, P, P]),
     'dtb_grad_rows_pack':(c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),

@@ -52,6 +52,21 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
+// The class DeepTable.predict gives a row of the model output: numpy's argmax of what predict_proba returns.  On one
+// column that is [1-p, p] (1 - p in float32), so class 1 when p > 1 - p; on several, the first maximum.
+__device__ __forceinline__ int predicted_class(const float* __restrict__ prob, int64_t r, int cols) {
+  if (cols == 1) {
+    const float p = prob[r];
+    return p > __fsub_rn(1.f, p) ? 1 : 0;
+  }
+  const float* pr = prob + r * cols;
+  int arg = 0;
+  float best = pr[0];
+  for (int c = 1; c < cols; ++c)
+    if (pr[c] > best) { best = pr[c]; arg = c; }
+  return arg;
+}
+
 // Streaming 16-byte load that does not pollute L1 (embedding rows are touched once per kernel).
 __device__ __forceinline__ float4 ldg_stream_f4(const float* p) {
   float4 r;

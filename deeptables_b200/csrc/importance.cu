@@ -92,22 +92,7 @@ __global__ void auc_finish_kernel(const unsigned long long* __restrict__ acc, in
   *out = (npos == 0.0 || nneg == 0.0) ? NAN : (rank2 - npos * (npos + 1.0)) / (2.0 * npos * nneg);
 }
 
-// ---- accuracy and F1 on predicted labels ---------------------------------------------------------------------------
-// The predicted class is numpy's argmax of what DeepTable.predict_proba returns: on one column, [1-p, p] (1 - p in
-// float32), so class 1 when p > 1 - p; on several, the first maximum.
-__device__ __forceinline__ int predicted_class(const float* __restrict__ prob, int64_t r, int cols) {
-  if (cols == 1) {
-    const float p = prob[r];
-    return p > __fsub_rn(1.f, p) ? 1 : 0;
-  }
-  const float* pr = prob + r * cols;
-  int arg = 0;
-  float best = pr[0];
-  for (int c = 1; c < cols; ++c)
-    if (pr[c] > best) { best = pr[c]; arg = c; }
-  return arg;
-}
-
+// ---- accuracy and F1 on predicted labels (predicted_class: dtb_common.cuh) ----------------------------------------
 // counters: [0] correct rows; then per class k: [1+k] TP, [1+K+k] predicted, [1+2K+k] true
 __global__ void label_count_kernel(const float* __restrict__ prob, const int* __restrict__ label, int64_t n, int cols,
                                    int classes, unsigned long long* __restrict__ acc) {

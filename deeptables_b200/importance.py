@@ -96,6 +96,20 @@ def permutation(rows, seed, iteration, column, device):
     return _sorted_keys(rows, seed, iteration, column, device) & 0xFFFFFFFF
 
 
+def forward_rows(model, cat, cont, pred, batch_size):
+    """The inference forward of ``model`` over the first ``len(pred)`` rows of the device inputs ``cat`` / ``cont``
+    (either may be None), ``batch_size`` rows per call, its outputs written into ``pred`` [rows, cols] float32.  The
+    caller brings the embedding rows up to date first (``model.flush_optimizer_state()``)."""
+    with torch.no_grad():
+        for lo in range(0, pred.shape[0], batch_size):
+            hi = min(lo + batch_size, pred.shape[0])
+            bc = cat[lo:hi] if cat is not None else None
+            bx = cont[lo:hi] if cont is not None else None
+            z = model._forward(bc, bx, training=False)
+            p, _ = E.loss_forward_backward(z, torch.zeros_like(z), model.task, None, False, None)
+            pred[lo:hi].copy_(p)
+
+
 def _class_ranks(labels):
     """Class code -> its position among the sorted labels (scikit-learn's column order for log loss and AUC)."""
     try:
@@ -187,13 +201,7 @@ def score_decreases(dt_model, X, y, metric, n_iter=5, mode='min', random_state=N
         states = torch.zeros(n_slots, state.state.numel(), dtype=torch.int64, device=device)
 
     def forward():
-        with torch.no_grad():
-            for lo in range(0, rows, batch_size):
-                bc = work['cat'][lo:lo + batch_size] if cat is not None else None
-                bx = work['cont'][lo:lo + batch_size] if cont is not None else None
-                z = model._forward(bc, bx, training=False)
-                p, _ = E.loss_forward_backward(z, torch.zeros_like(z), model.task, None, False, None)
-                pred[lo:lo + p.shape[0]].copy_(p)
+        forward_rows(model, work['cat'], work['cont'], pred, batch_size)
 
     def score(slot):
         out = _ptr_at(scores, slot)

@@ -384,6 +384,25 @@ int dtb_importance_labels(int metric, const float* prob, const int* label, int64
 int dtb_importance_sums(int metric, const float* prob, const int* label, const double* target, int64_t rows, int cols,
                         double aux, void* scratch, double* out, void* stream);
 
+/* ---- Kernel SHAP (deeptables_b200/explain.py, utils/shap.py) ----------------------------------------------------- */
+/* The synthetic rows of `coalitions` coalitions over `bg_rows` background rows: row k*bg_rows + j is background row j
+ * (bg_cat [bg_rows, fields], bg_cont [bg_rows, conts]) with every column whose bit is set in mask k replaced by the
+ * value of explained row x_index[k] (x_cat [*, fields], x_cont [*, conts]).  masks: [coalitions, mask_words] bit sets;
+ * cat_bit[f] / cont_bit[c]: the column's bit, or -1 for a column that always keeps the background's value.  Writes
+ * out_cat [coalitions*bg_rows, fields] and out_cont [coalitions*bg_rows, conts]; fields or conts may be 0 (then their
+ * pointers may be NULL). */
+int dtb_shap_compose(const int32_t* x_cat, const float* x_cont, const int32_t* bg_cat, const float* bg_cont,
+                     const uint32_t* masks, int mask_words, const int32_t* x_index, const int32_t* cat_bit,
+                     const int32_t* cont_bit, int64_t coalitions, int bg_rows, int fields, int conts,
+                     int32_t* out_cat, float* out_cont, void* stream);
+/* out[g] (float64) = the mean, over rows g*rows_per_group .. +rows_per_group-1 of the model output prob [*, cols], of
+ * the model function: the output itself (DTB_SHAP_VALUE, one column) or DeepTable.predict's class code
+ * (DTB_SHAP_CLASS: p > 1 - p in float32 on one column, the first arg-max on several).  Fixed summation order. */
+#define DTB_SHAP_VALUE 0
+#define DTB_SHAP_CLASS 1
+int dtb_shap_means(const float* prob, int64_t groups, int rows_per_group, int cols, int kind, double* out,
+                   void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
