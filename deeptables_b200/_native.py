@@ -53,6 +53,24 @@ class LossParams(ctypes.Structure):
 
 _LPP = POINTER(LossParams)
 
+
+class GbdtSplitRec(ctypes.Structure):
+    """``dtb_gbdt_split_rec``: a leaf's integer sums and its best split (feature -1: none)."""
+    _fields_ = [('gain', c_double), ('g', c_int64), ('h', c_int64), ('left_g', c_int64), ('left_h', c_int64),
+                ('count', ctypes.c_int32), ('left_count', ctypes.c_int32), ('feature', ctypes.c_int32),
+                ('bin', ctypes.c_int32)]
+
+
+class GbdtSplitParams(ctypes.Structure):
+    """``dtb_gbdt_split_params`` (host memory, read at call time)."""
+    _fields_ = [('lambda_l2', c_double), ('lambda_l1', c_double), ('min_split_gain', c_double),
+                ('min_child_weight', c_double), ('scale_g', c_double), ('scale_h', c_double),
+                ('min_child_samples', ctypes.c_int32)]
+
+
+GBDT_BINARY, GBDT_L2, GBDT_SOFTMAX = 0, 1, 2
+GBDT_STAGE_NODES = 2048
+
 _SIGNATURES = {
     'dtb_version': (c_int, []),
     'dtb_last_error': (c_char_p, []),
@@ -118,6 +136,15 @@ _SIGNATURES = {
     'dtb_importance_sums': (c_int, [c_int, P, P, P, c_int64, c_int, c_double, P, P, P]),
     'dtb_shap_compose': (c_int, [P, P, P, P, P, c_int, P, P, P, c_int64, c_int, c_int, c_int, P, P, P]),
     'dtb_shap_means': (c_int, [P, c_int64, c_int, c_int, c_int, P, P]),
+    'dtb_gbdt_bin': (c_int, [P, c_int, P, c_int, P, P, P, c_int64, c_int, P, P]),
+    'dtb_gbdt_grad': (c_int, [P, P, c_int64, c_int, c_int, c_int, P, P, P, P]),
+    'dtb_gbdt_fixed': (c_int, [P, P, c_int64, c_int, c_int, P, P, P]),
+    'dtb_gbdt_hist': (c_int, [P, P, c_int64, c_int64, P, P, c_int, c_int, P, P, P, P]),
+    'dtb_gbdt_hist_sub': (c_int, [P, P, P, P, P, P, c_int64, c_int, P]),
+    'dtb_gbdt_split': (c_int, [P, P, P, P, c_int, P, c_int, c_int, POINTER(GbdtSplitParams), P, P]),
+    'dtb_gbdt_partition': (c_int, [P, c_int, P, c_int64, c_int64, c_int, c_int, c_int64, P, P]),
+    'dtb_gbdt_update': (c_int, [P, P, P, c_int, c_int64, P, P, c_int, c_int, P, c_int64, P]),
+    'dtb_gbdt_leaves': (c_int, [P, c_int, P, c_int, P, P, P, P, P, P, c_int, c_int, c_int64, P, P, c_int, c_int, P]),
     'dtb_grad_rows_pack':(c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),

@@ -6,8 +6,9 @@ layer that makes the README flow work on a pandas DataFrame: a pandas/sklearn ``
 with the reference's column conventions (label-encoded categoricals with ``nunique + 2`` vocabulary
 slots, reference preprocessor.py:333; one continuous group named ``input_continuous_all``,
 preprocessor.py:495-500), early stopping injected as the reference does (deeptable.py:709-754) and
-the binary ``[1-p, p]`` probability fix (deeptable.py:689-691).  Cross-validation, GBM features,
-discretisation, var-len columns and the model-set leaderboard are out of scope (SURVEY.md 8f).
+the binary ``[1-p, p]`` probability fix (deeptable.py:689-691), and the gradient-boosted leaf columns of
+``apply_gbm_features`` (gbm.py).  Discretisation, var-len columns and the model-set leaderboard are out of scope
+(SURVEY.md 8f).
 """
 import copy
 import os
@@ -114,6 +115,9 @@ class DefaultPreprocessor:
             y = y.astype(np.float32)
         X = X.drop(columns=[c for c in (self.config.exclude_columns or []) if c in X.columns])
         cfg = self.config
+        if cfg.apply_gbm_features:
+            from .gbm import GbmLeavesEncoder
+            GbmLeavesEncoder.check_names(X)
         cats, conts = [], []
         for c in X.columns:
             col = X[c]
@@ -149,11 +153,41 @@ class DefaultPreprocessor:
             d = dim if cfg.fixed_embedding_dim else min(4 * int(pow(vocab, 0.25)), 20)
             self.categorical_columns.append(CategoricalColumn(c, vocab, d))
         self.continuous_columns = [ContinuousColumn('input_continuous_all', list(conts))] if conts else []
-        Xt = self.transform_X(X)
+        self.gbm_encoder_ = None
+        Xt = self._encode(X)
+        if cfg.apply_gbm_features and y is not None:
+            Xt = self._fit_gbm_features(Xt, y, dim)
         self.fit_seconds_ = time.time() - t0
         return Xt, y
 
+    def _fit_gbm_features(self, Xt, y, dim):
+        """The reference's _apply_gbm_features (preprocessor.py:431-452): trees on the encoded, imputed and scaled
+        columns; one embedded column per tree, or one continuous group holding the raw leaf indices."""
+        from . import gbm
+        cfg = self.config
+        if self.task_ == consts.TASK_MULTILABEL:
+            raise NotImplementedError('apply_gbm_features on the multilabel task')
+        enc = gbm.GbmLeavesEncoder(self._cat_names, self._cont_names, self.task_, **(cfg.gbm_params or {}))
+        Xt = enc.fit_transform(Xt, y, len(self.labels_) if self.labels_ else None)
+        self.gbm_encoder_ = enc
+        if cfg.gbm_feature_type == consts.GBM_FEATURE_TYPE_EMB:
+            for name, leaves in zip(enc.new_columns, enc.trees.num_leaves):
+                vocab = int(leaves)           # every leaf holds training rows: the reference's max + 1
+                d = dim if cfg.fixed_embedding_dim else min(4 * int(pow(vocab, 0.25)), 20)
+                self.categorical_columns.append(CategoricalColumn(name, vocab, d))
+        elif enc.new_columns:
+            self.continuous_columns.append(ContinuousColumn(consts.INPUT_PREFIX_NUM + 'gbm_leaves',
+                                                            list(enc.new_columns)))
+        return Xt
+
     def transform_X(self, X):
+        enc = getattr(self, 'gbm_encoder_', None)
+        if enc is not None:
+            enc.check_names(X)
+        Xt = self._encode(X)
+        return enc.transform(Xt) if enc is not None else Xt
+
+    def _encode(self, X):
         X = X.copy()
         X.columns = [str(c) for c in X.columns]
         out = {}

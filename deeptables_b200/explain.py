@@ -8,7 +8,8 @@ are computed here: the frames are encoded and uploaded once, ``dtb_shap_compose`
 of coalitions (of several explained rows at once), the inference forward runs over them in batches and
 ``dtb_shap_means`` reduces each coalition's rows into one float64.  The host reads the values once per group of
 explained rows and solves shap's constrained weighted least squares in float64.  DefaultPreprocessor encodes each cell
-on its own, so composing encoded columns is composing raw ones.
+on its own, so composing encoded columns is composing raw ones.  Gradient-boosted leaf columns are not columns of X:
+they get no SHAP column and are recomputed from each composed row on the device.
 
 The model function is ``DeepTable.predict(X, encode_to_label=False)``: the prediction on regression, the class code
 otherwise.  The draws of row i come from ``np.random.RandomState([seed, i])``, so a given seed gives the same bits for
@@ -24,7 +25,7 @@ from math import comb
 import numpy as np
 import torch
 
-from . import _native as N, consts, dp
+from . import _native as N, consts, dp, gbm
 from ._native import check, ptr, stream_ptr
 from .importance import forward_rows
 
@@ -289,6 +290,7 @@ def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, t
             check(N.lib.dtb_shap_compose(ptr(x_cat), ptr(x_cont), ptr(bg.cat), ptr(bg.cont), ptr(masks_dev[k0:]),
                                          bg.words, ptr(index_dev[k0:]), ptr(bg.cat_bit), ptr(bg.cont_bit), k, N_bg,
                                          F, C, ptr(out_cat), ptr(out_cont), stream_ptr()), 'shap_compose')
+            gbm.rewrite_leaves(bg.dt_model.preprocessor, out_cat[:rows] if F else None, out_cont[:rows] if C else None)
             if timer:
                 end.record()
                 end = timer.device('forward')

@@ -4,7 +4,8 @@ The frame is encoded by the preprocessor and uploaded once; a pass permutes the 
 copy of the model's inputs (``dtb_perm_keys`` + ``torch.sort`` + ``dtb_shuffle_column``), runs the inference forward
 over the copy in batches, scores the predictions into one float64 slot of a device array and puts the column back.
 The host reads the slots once, after the last pass.  DefaultPreprocessor encodes each column on its own and row by
-row, so permuting an encoded column is permuting the raw one.
+row, so permuting an encoded column is permuting the raw one.  Gradient-boosted leaf columns (``apply_gbm_features``)
+are recomputed from the permuted columns on the device; they are not columns of X, so they get no importance.
 
 Data parallel: every rank calls this with the same frame; pass ``s`` (0 is the unpermuted base) runs on rank
 ``s % world`` and the slots are all-gathered, so every rank returns what one process would.
@@ -16,7 +17,7 @@ import numbers
 import numpy as np
 import torch
 
-from . import _native as N, consts, dp, engine as E, metrics as M
+from . import _native as N, consts, dp, engine as E, gbm, metrics as M
 from ._native import check, ptr, stream_ptr
 
 AUC, LOG_LOSS, ACCURACY, F1, F1_MACRO, MSE, RMSE, MAE, R2 = range(1, 10)     # DTB_IMPORTANCE_* (deeptables_b200.h)
@@ -236,9 +237,11 @@ def score_decreases(dt_model, X, y, metric, n_iter=5, mode='min', random_state=N
             perm = _sorted_keys(rows, seed, it, j, device)
             check(N.lib.dtb_shuffle_column(ptr(src[key]), ptr(arr), ptr(perm), rows, arr.shape[1], col, stream_ptr()),
                   'shuffle_column')
+            gbm.rewrite_leaves(dt_model.preprocessor, work['cat'], work['cont'])
             forward()
             check(N.lib.dtb_shuffle_column(ptr(src[key]), ptr(arr), None, rows, arr.shape[1], col, stream_ptr()),
                   'shuffle_column')
+            gbm.rewrite_leaves(dt_model.preprocessor, work['cat'], work['cont'])
             passes += 1
         score(slot)
 

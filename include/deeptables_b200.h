@@ -403,6 +403,74 @@ int dtb_shap_compose(const int32_t* x_cat, const float* x_cont, const int32_t* b
 int dtb_shap_means(const float* prob, int64_t groups, int rows_per_group, int cols, int kind, double* out,
                    void* stream);
 
+/* ---- gradient-boosted leaf features (deeptables_b200/gbm.py; reference preprocessor.py:431-452) ------------------- */
+/* Feature i of a booster is read from the model's own inputs: feat_col[i] = c >= 0 is column c of cat [rows, cat_stride]
+ * (int32 codes, compared as their float32 values), feat_col[i] = -1 - c is column c of cont [rows, cont_stride].
+ * edges (float32) holds each feature's increasing bin edges at edge_off[i] .. edge_off[i+1]-1; the bin of x is the
+ * number of edges < x, NaN the last bin (the number of edges).  bins [rows, nf] uint8, row-major. */
+int dtb_gbdt_bin(const int32_t* cat, int cat_stride, const float* cont, int cont_stride, const int32_t* feat_col,
+                 const float* edges, const int32_t* edge_off, int64_t rows, int nf, uint8_t* bins, void* stream);
+/* Gradient and hessian of class k of the float64 scores [rows, K] (LightGBM's objectives): DTB_GBDT_BINARY p - y,
+ * p(1-p) with p = sigmoid(s); DTB_GBDT_L2 s - y, 1; DTB_GBDT_SOFTMAX p_k - [y = k], K/(K-1) p_k(1-p_k).  Computed in
+ * float64, rounded to float32 into g, h; label is float32 (binary, L2) or the class code as float32 (softmax).
+ * max_gh[0..1] (device, caller zeroes) receive max |g| and max h by integer atomics on their bit patterns. */
+#define DTB_GBDT_BINARY 0
+#define DTB_GBDT_L2 1
+#define DTB_GBDT_SOFTMAX 2
+int dtb_gbdt_grad(const double* scores, const float* label, int64_t rows, int K, int k, int objective, float* g,
+                  float* h, float* max_gh, void* stream);
+/* Fixed point: gq = rint(g * 2^shift_g), hq = rint(h * 2^shift_h) as int64 (the caller picks the shifts so that no
+ * sum over rows reaches 2^62). */
+int dtb_gbdt_fixed(const float* g, const float* h, int64_t rows, int shift_g, int shift_h, int64_t* gq, int64_t* hq,
+                   void* stream);
+/* Histogram of one leaf: the rows index[begin .. begin+count) of bins.  hist_g / hist_h (int64) and hist_n (int32),
+ * each [nf, nb] (nb >= every feature's bin count, <= 256), are overwritten with the sums of gq, hq and the row count
+ * per (feature, bin).  Integer sums: the result does not depend on the order of the rows. */
+int dtb_gbdt_hist(const uint8_t* bins, const int32_t* index, int64_t begin, int64_t count, const int64_t* gq,
+                  const int64_t* hq, int nf, int nb, int64_t* hist_g, int64_t* hist_h, int32_t* hist_n, void* stream);
+/* The subtraction trick on [elements] of the three arrays, leaving the left child in parent_* and the right one in
+ * small_*: small_is_left = 0 (small holds the right child): parent -= small; small_is_left = 1: (parent, small) =
+ * (small, parent - small). */
+int dtb_gbdt_hist_sub(int64_t* parent_g, int64_t* parent_h, int32_t* parent_n, int64_t* small_g, int64_t* small_h,
+                      int32_t* small_n, int64_t elements, int small_is_left, void* stream);
+/* Best split of each leaf in leaves[0 .. n_leaves): the histogram of leaf l is hist_* + l * nf * nb.  Candidate
+ * (feature f, bin t < n_bins[f] - 1) sends bins <= t left.  Valid when both sides have >= min_child_samples rows and a
+ * hessian >= min_child_weight; gain in float64 from the integer sums (G = gq_sum * scale_g, H = hq_sum * scale_h),
+ * T(G)^2/(H+lambda) left + right - parent - min_split_gain, T the L1 soft threshold at alpha; ties to the lowest
+ * feature, then the lowest t.  out[i] gets the leaf's sums and its best split (feature -1, gain 0 when none has
+ * gain > 0). */
+typedef struct {
+  double gain;
+  int64_t g, h, left_g, left_h;
+  int32_t count, left_count, feature, bin;
+} dtb_gbdt_split_rec;
+typedef struct {
+  double lambda_l2, lambda_l1, min_split_gain, min_child_weight, scale_g, scale_h;
+  int32_t min_child_samples;
+} dtb_gbdt_split_params;
+int dtb_gbdt_split(const int64_t* hist_g, const int64_t* hist_h, const int32_t* hist_n, const int32_t* leaves,
+                   int n_leaves, const int32_t* n_bins, int nf, int nb, const dtb_gbdt_split_params* params_host,
+                   dtb_gbdt_split_rec* out, void* stream);
+/* Split the segment index[begin .. begin+count) in place: rows whose bin of `feature` is <= bin first (left_count of
+ * them, from the split record), the rest after; the order inside each half is unspecified.  scratch: int32 [count + 2]. */
+int dtb_gbdt_partition(const uint8_t* bins, int nf, int32_t* index, int64_t begin, int64_t count, int feature,
+                       int bin, int64_t left_count, int32_t* scratch, void* stream);
+/* After a tree: for every leaf l, each row r of index[seg_begin[l] .. + seg_count[l]) gets
+ * scores[r * K + k] += (double)leaf_value[l] and, when leaf_out is not NULL, leaf_out[r * leaf_stride] = l. */
+int dtb_gbdt_update(const int32_t* index, const int64_t* seg_begin, const int64_t* seg_count, int n_leaves,
+                    int64_t max_count, const float* leaf_value, double* scores, int K, int k, int32_t* leaf_out,
+                    int64_t leaf_stride, void* stream);
+/* Leaf index of every row in each of n_trees trees, walked on the raw values (x <= threshold goes left, NaN right).
+ * Tree t's internal nodes are node_* [node_off[t] .. node_off[t+1]); a child >= 0 is a node of the same tree, a child
+ * < 0 the leaf ~child; a tree without nodes is the single leaf 0.  Trees are staged in shared memory in chunks of at
+ * most DTB_GBDT_STAGE_NODES nodes (a larger tree is refused).  Leaf j of tree t goes to out_cat[r * out_stride +
+ * out_col + t] (int32) when out_cat is not NULL, else to out_cont[...] as float32. */
+#define DTB_GBDT_STAGE_NODES 2048
+int dtb_gbdt_leaves(const int32_t* cat, int cat_stride, const float* cont, int cont_stride, const int32_t* feat_col,
+                    const int32_t* node_feature, const float* node_threshold, const int32_t* node_left,
+                    const int32_t* node_right, const int32_t* node_off, int n_trees, int max_tree_nodes,
+                    int64_t rows, int32_t* out_cat, float* out_cont, int out_stride, int out_col, void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
