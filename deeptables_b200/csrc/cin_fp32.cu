@@ -5,7 +5,7 @@
 // are needed, materialises the outer product Z only for a bounded chunk of batch rows, and runs the
 // GEMMs as plain fp32 library GEMMs.  It is the any-shape path (odd D, odd layer sizes, direct=True
 // with wide layers, ...) and the high-precision GPU cross-check for the tensor-core kernel in
-// cin_tc.cu, which is the product path for the shapes it supports.
+// cin_wgmma.cu, which is the product path for the shapes it supports.
 //
 //   x0t[b,d,i]            = E[b,i,d]                       (gather fused into the transpose)
 //   Z_k[(b,d), i*H_k + j] = x0t[b,d,i] * h_k[b,d,j]        (layers.py:690-695)

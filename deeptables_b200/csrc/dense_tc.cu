@@ -4,7 +4,7 @@
 //
 // fp32 in, fp32 out.  Operands are split on the fly into bf16 hi + lo and multiplied in three tensor passes
 // (hi*hi + lo*hi + hi*lo, fp32 accumulation): each operand is represented to 2^-18, the dropped lo*lo term is
-// 2^-18 of a product, i.e. fp32-grade results (the same scheme the CIN kernels use, cin_tc.cu).
+// 2^-18 of a product, i.e. fp32-grade results (the same scheme the CIN kernels use, cin_wgmma.cu).
 //
 //   rows kernel   out[M, Nout] = act(A[M, K] . W + bias)       W given as packed images (dense_tc_pack_kernel)
 //                 forward:   A = X,  W = kernel          [K = in_dim,  Nout = out_dim]

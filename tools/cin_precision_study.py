@@ -1,6 +1,6 @@
 """CPU study: which operand splits keep the CIN feature-map GEMMs inside the 1e-3 parity bar?
 
-Emulates the tensor-core arithmetic of cin_tc_fwd_kernel (operands rounded to a 16-bit format, exact products,
+Emulates split-operand tensor-core GEMMs (each fp32 operand rounded to one or two 16-bit terms, exact products,
 fp32-or-better accumulation) for the xDeepFM CIN (26 fields x 16, 128x128x128, half-split) on random rows and
 compares the pooled feature maps with a float64 evaluation.  Schemes: bf16 x1 / x3 (the product path), fp16 x1,
 fp16 x2 with the on-the-fly operand Z split (Z_hi W + Z_lo W) or the weights split (Z W_hi + Z W_lo), all with
