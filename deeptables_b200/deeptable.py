@@ -6,9 +6,9 @@ layer that makes the README flow work on a pandas DataFrame: a pandas/sklearn ``
 with the reference's column conventions (label-encoded categoricals with ``nunique + 2`` vocabulary
 slots, reference preprocessor.py:333; one continuous group named ``input_continuous_all``,
 preprocessor.py:495-500), early stopping injected as the reference does (deeptable.py:709-754) and
-the binary ``[1-p, p]`` probability fix (deeptable.py:689-691), and the gradient-boosted leaf columns of
-``apply_gbm_features`` (gbm.py).  Discretisation, var-len columns and the model-set leaderboard are out of scope
-(SURVEY.md 8f).
+the binary ``[1-p, p]`` probability fix (deeptable.py:689-691), the quantile-bin columns of ``auto_discrete``
+(discrete.py) and the gradient-boosted leaf columns of ``apply_gbm_features`` (gbm.py).  Var-len columns and the
+model-set leaderboard are out of scope (SURVEY.md 8f).
 """
 import copy
 import os
@@ -154,20 +154,41 @@ class DefaultPreprocessor:
             self.categorical_columns.append(CategoricalColumn(c, vocab, d))
         self.continuous_columns = [ContinuousColumn('input_continuous_all', list(conts))] if conts else []
         self.gbm_encoder_ = None
+        self.discretizer_ = None
+        if cfg.auto_discrete and conts:
+            from .discrete import MultiKBinsDiscretizer
+            MultiKBinsDiscretizer.check_names(X, conts)
         Xt = self._encode(X)
+        if cfg.auto_discrete and conts:
+            Xt = self._fit_discretizer(Xt, dim)
         if cfg.apply_gbm_features and y is not None:
             Xt = self._fit_gbm_features(Xt, y, dim)
         self.fit_seconds_ = time.time() - t0
         return Xt, y
 
+    def _fit_discretizer(self, Xt, dim):
+        """The reference's _discretization (preprocessor.py:406-415): one quantile-bin code per continuous column,
+        appended after the label-encoded categoricals as an embedded column of vocabulary n_bins + 1."""
+        from .discrete import MultiKBinsDiscretizer
+        disc = MultiKBinsDiscretizer(self._cont_names)
+        Xt = disc.fit_transform(Xt)
+        self.discretizer_ = disc
+        for name, vocab in zip(disc.new_columns, disc.vocabulary_sizes):
+            d = dim if self.config.fixed_embedding_dim else min(4 * int(pow(vocab, 0.25)), 20)
+            self.categorical_columns.append(CategoricalColumn(name, vocab, d))
+        return Xt
+
     def _fit_gbm_features(self, Xt, y, dim):
         """The reference's _apply_gbm_features (preprocessor.py:431-452): trees on the encoded, imputed and scaled
-        columns; one embedded column per tree, or one continuous group holding the raw leaf indices."""
+        columns, the discretised ones among the categorical inputs; one embedded column per tree, or one continuous
+        group holding the raw leaf indices."""
         from . import gbm
         cfg = self.config
         if self.task_ == consts.TASK_MULTILABEL:
             raise NotImplementedError('apply_gbm_features on the multilabel task')
-        enc = gbm.GbmLeavesEncoder(self._cat_names, self._cont_names, self.task_, **(cfg.gbm_params or {}))
+        disc = self.discretizer_
+        enc = gbm.GbmLeavesEncoder(self._cat_names + (disc.new_columns if disc is not None else []), self._cont_names,
+                                   self.task_, **(cfg.gbm_params or {}))
         Xt = enc.fit_transform(Xt, y, len(self.labels_) if self.labels_ else None)
         self.gbm_encoder_ = enc
         if cfg.gbm_feature_type == consts.GBM_FEATURE_TYPE_EMB:
@@ -182,9 +203,14 @@ class DefaultPreprocessor:
 
     def transform_X(self, X):
         enc = getattr(self, 'gbm_encoder_', None)
+        disc = getattr(self, 'discretizer_', None)
         if enc is not None:
             enc.check_names(X)
+        if disc is not None:
+            disc.check_names(X, disc.columns)
         Xt = self._encode(X)
+        if disc is not None:
+            Xt = disc.transform(Xt)
         return enc.transform(Xt) if enc is not None else Xt
 
     def _encode(self, X):

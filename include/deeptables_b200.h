@@ -471,6 +471,15 @@ int dtb_gbdt_leaves(const int32_t* cat, int cat_stride, const float* cont, int c
                     const int32_t* node_right, const int32_t* node_off, int n_trees, int max_tree_nodes,
                     int64_t rows, int32_t* out_cat, float* out_cont, int out_stride, int out_col, void* stream);
 
+/* ---- quantile-bin discretisation (deeptables_b200/discrete.py; reference preprocessor.py:406-415) ------------------ */
+/* out_cat[r * out_stride + out_col + j] (int32) = the number of inner edges e of column j with e <= (double)x, where
+ * x = cont[r * cont_stride + src_col[j]] (numpy's searchsorted side='right': ties go to the upper bin, -0.0 == 0.0).
+ * Column j's increasing float64 inner edges are edges[edge_off[j] .. edge_off[j+1]); a column without edges gets
+ * code 0.  src_col[j] < cont_stride is the caller's to guarantee (device memory).  One launch covers every row and
+ * column, with 64-bit indexing; the edges are searched in global memory, so a column may have any number of them. */
+int dtb_discretize(const float* cont, int cont_stride, int64_t rows, const int32_t* src_col, const double* edges,
+                   const int64_t* edge_off, int n_cols, int32_t* out_cat, int out_stride, int out_col, void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
