@@ -24,8 +24,45 @@ Every function takes/returns torch tensors on CPU; dtype follows the inputs (flo
 reference, float64 gives a high-precision check), and autograd through these functions is the
 backward oracle.
 """
+import contextlib
 import math
+import sys
 import torch
+
+# ---------------------------------------------------------------------------------------------
+# Optional record of the relu and max decisions a forward pass takes (off unless `recording` installs a list).
+# A float32 forward can decide an entry the other way where the float64 input lies within rounding of the
+# threshold or of the runner-up; a gradient check needs to know which entries those are.
+# ---------------------------------------------------------------------------------------------
+_recorder = None
+
+
+@contextlib.contextmanager
+def recording(entries):
+    """While active, every relu (`activation(..., 'relu')`, the bare relus of multihead_attention and senet) and every
+    max (SENET's amax, each maxpool_fields window) appends (site, x, y, dim) to `entries`: the input x, the output y
+    and the reduced axis of a max (None for a relu).  site names the oracle function that took the decision."""
+    global _recorder
+    prev, _recorder = _recorder, entries
+    try:
+        yield entries
+    finally:
+        _recorder = prev
+
+
+def _decision(x, y, dim=None):
+    if _recorder is None:
+        return y
+    frame = sys._getframe(1)
+    while frame.f_code.co_name in ('_decision', 'activation', 'dense', 'relu'):
+        frame = frame.f_back
+    _recorder.append((frame.f_code.co_name, x, y, dim))
+    return y
+
+
+def relu(x):
+    return _decision(x, torch.relu(x))
+
 
 # ---------------------------------------------------------------------------------------------
 # Keras-default facts the reference relies on implicitly (SURVEY.md section 8c)
@@ -41,7 +78,7 @@ def activation(x, name):
     if name is None or name == 'linear':
         return x
     if name == 'relu':
-        return torch.relu(x)
+        return relu(x)
     if name == 'sigmoid':
         return torch.sigmoid(x)
     if name == 'tanh':
@@ -257,7 +294,7 @@ def multihead_attention(x, params, weights, bn_state, training):
     out = torch.cat(torch.chunk(out, num_heads, dim=0), dim=2)
     if use_residual:
         out = out + v_res
-    out = torch.relu(out)
+    out = relu(out)
     y, nm, nv = batch_norm(out, weights['batch_normalize/gamma'], weights['batch_normalize/beta'],
                            bn_state['moving_mean'], bn_state['moving_variance'], training)
     return y, {'moving_mean': nm, 'moving_variance': nv}
@@ -331,9 +368,10 @@ def senet(x, att1_kernel, att1_bias, att2_kernel, att2_bias, pooling_op='mean'):
     A = relu(Dense(F)(relu(Dense(max(F // reduction_ratio, 1))(Z)))); V = x * A[:, :, None]."""
     if x.dim() != 3:
         raise ValueError(f'Wrong dimensions of inputs, expected 3 but input {x.dim()}.')
-    z = x.amax(dim=-1) if pooling_op == 'max' else x.mean(dim=-1)       # amax: ties share the gradient, as tf.reduce_max does
-    a1 = torch.relu(z @ att1_kernel + att1_bias)
-    a2 = torch.relu(a1 @ att2_kernel + att2_bias)
+    # amax: ties share the gradient, as tf.reduce_max does
+    z = _decision(x, x.amax(dim=-1), -1) if pooling_op == 'max' else x.mean(dim=-1)
+    a1 = relu(z @ att1_kernel + att1_bias)
+    a2 = relu(a1 @ att2_kernel + att2_bias)
     return x * a2.unsqueeze(2)
 
 
@@ -382,7 +420,8 @@ def maxpool_fields(x, pool):
     rows = []
     for o in range(out):
         lo, hi = max(o * pool - before, 0), min(o * pool - before + pool, x.shape[1])
-        rows.append(x[:, lo:hi].max(dim=1).values)        # the gradient goes to the first maximum (TensorFlow's MaxPoolGrad argmax)
+        win = x[:, lo:hi]
+        rows.append(_decision(win, win.max(dim=1).values, 1))   # the gradient goes to the first maximum (TensorFlow's MaxPoolGrad argmax)
     return torch.stack(rows, dim=1)
 
 
