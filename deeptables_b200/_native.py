@@ -146,6 +146,7 @@ _SIGNATURES = {
     'dtb_gbdt_update': (c_int, [P, P, P, c_int, c_int64, P, P, c_int, c_int, P, c_int64, P]),
     'dtb_gbdt_leaves': (c_int, [P, c_int, P, c_int, P, P, P, P, P, P, c_int, c_int, c_int64, P, P, c_int, c_int, P]),
     'dtb_discretize': (c_int, [P, c_int, c_int64, P, P, P, c_int, P, c_int, c_int, P]),
+    'dtb_dae_swap_batch': (c_int, [P, c_int, P, P, P, P, c_int, c_int, c_int, c_ulonglong, P, P, P]),
     'dtb_grad_rows_pack':(c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_grad_rows_unpack': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_cin_saved_bytes': (c_size_t, [c_int, c_int, c_int, _IP, c_int, c_int]),

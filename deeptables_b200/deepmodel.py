@@ -625,10 +625,8 @@ class DeepModel:
             if dev_step:
                 check(N.lib.dtb_step_increment(ptr(self._step_dev), stream_ptr()), 'step_increment')
             return prob
+        dense_step(scope, o, None, self._rates, step, self._step_dev if dev_step else None)
         if dev_step:
-            check(N.lib.dtb_adam_dense_dev(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
-                                           scope.flat_p.numel(), ptr(self._rates.dev), ptr(self._step_dev), o.beta_1,
-                                           o.beta_2, o.epsilon, 1, stream_ptr()), 'adam_dense_dev')
             if t is not None:
                 if t.lazy_active:
                     check(N.lib.dtb_adam_rows_apply_dev(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m), ptr(t.v),
@@ -648,9 +646,6 @@ class DeepModel:
             check(N.lib.dtb_step_increment(ptr(self._step_dev), stream_ptr()), 'step_increment')
             return prob
         alpha = float(self._rates.host[step])          # the float32 the CUDA-graph form reads from the table
-        check(N.lib.dtb_adam_dense(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
-                                   scope.flat_p.numel(), alpha, o.beta_1, o.beta_2, o.epsilon, 1,
-                                   stream_ptr()), 'adam_dense')
         if t is not None:
             if t.lazy_active:
                 check(N.lib.dtb_adam_rows_apply(ptr(union_cat), ptr(t.row_offsets), ptr(t.weight), ptr(t.m),
@@ -673,11 +668,10 @@ class DeepModel:
         update (lazy) or dense sweep (with the table's regularization fused in; `rows` scales its loss term).  Each
         reads the step's rate from the rate table: at `step`, or in the CUDA-graph form at the device counter + 1."""
         scope, t, hp = self._scope, self.table, self._opt_native
-        lr = (ptr(self._rates.dev), 0, ptr(self._step_dev)) if dev_step else (ptr(self._rates.dev), step, None)
-        check(N.lib.dtb_optim_dense_lr(ptr(scope.flat_p), ptr(scope.flat_g), *[ptr(x) for x in scope.flat_slots],
-                                       scope.flat_p.numel(), hp, *lr, 1, stream_ptr()), 'optim_dense_lr')
+        dense_step(scope, self._opt, hp, self._rates, step, self._step_dev if dev_step else None)
         if t is None:
             return
+        lr = (ptr(self._rates.dev), 0, ptr(self._step_dev)) if dev_step else (ptr(self._rates.dev), step, None)
         s = [ptr(x) for x in t.slots]
         if self._emb_reg is not None:
             r = self._emb_reg
@@ -739,27 +733,19 @@ class DeepModel:
             sx = None if cont is None else torch.empty_like(cont)
             sy = torch.empty_like(y)
             self._step_dev.fill_(self._step)
-            try:
-                import gc
-                gc.collect()             # no autograd graph of an earlier (eager) step may outlive into the capture
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                l0 = N.lib.dtb_launch_count()
-                with self._scope.device_seeds() as seeds, torch.cuda.graph(graph):
-                    prob = self._train_step_body(sc, sx, sy, None, dev_step=True)
-                    if seeds is not None:
-                        check(N.lib.dtb_seed_advance(ptr(seeds), seeds.numel(), stream_ptr()), 'seed_advance')
-                n_launch = N.lib.dtb_launch_count() - l0          # kernels of this library inside one replay
-            except Exception as exc:                       # capture unsupported here: say so once, run eagerly from now on
+
+            def body(seeds):
+                prob = self._train_step_body(sc, sx, sy, None, dev_step=True)
+                if seeds is not None:
+                    check(N.lib.dtb_seed_advance(ptr(seeds), seeds.numel(), stream_ptr()), 'seed_advance')
+                return prob
+            captured = capture_step(body, self._scope.device_seeds)
+            if captured is None:                           # capture unsupported here: run eagerly from now on
                 self._graph_failed = True
-                import warnings
-                warnings.warn(f'deeptables_b200: CUDA-graph capture of the train step failed ({type(exc).__name__}: {exc}); '
-                              f'continuing with eager launches')
-                torch.cuda.synchronize()
                 prob = self._train_step_body(cat, cont, y, None, dev_step=False)
                 self._step += 1
                 return prob
-            N.lib.dtb_launch_count_add(-n_launch)                # counted at capture, not executed yet
+            graph, prob, n_launch = captured
             entry = self._graphs[key] = (graph, sc, sx, sy, prob, n_launch)
         graph, sc, sx, sy, prob, n_launch = entry
         if sc is not None:
@@ -1487,6 +1473,47 @@ class _ModelOptimizer:
 
     def __repr__(self):
         return f'<{self._model._opt.keras_name} learning_rate={self.learning_rate} iterations={self.iterations}>'
+
+
+def dense_step(scope, opt, hp, rates, step, step_dev=None):
+    """Optimiser step ``step`` over the flat parameters of a frozen ``_Scope``, zeroing their gradient: Adam through
+    dtb_adam_dense, SGD / RMSprop / Adagrad (``hp``: their dtb_optim_params) through dtb_optim_dense_lr, at the rate of
+    the ``_StepRates`` table.  With ``step_dev`` (the CUDA-graph form) the kernels read the step as *step_dev + 1."""
+    if opt.kind != 'adam':
+        lr = (ptr(rates.dev), 0, ptr(step_dev)) if step_dev is not None else (ptr(rates.dev), step, None)
+        check(N.lib.dtb_optim_dense_lr(ptr(scope.flat_p), ptr(scope.flat_g), *[ptr(x) for x in scope.flat_slots],
+                                       scope.flat_p.numel(), hp, *lr, 1, stream_ptr()), 'optim_dense_lr')
+    elif step_dev is not None:
+        check(N.lib.dtb_adam_dense_dev(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
+                                       scope.flat_p.numel(), ptr(rates.dev), ptr(step_dev), opt.beta_1, opt.beta_2,
+                                       opt.epsilon, 1, stream_ptr()), 'adam_dense_dev')
+    else:
+        check(N.lib.dtb_adam_dense(ptr(scope.flat_p), ptr(scope.flat_m), ptr(scope.flat_v), ptr(scope.flat_g),
+                                   scope.flat_p.numel(), float(rates.host[step]), opt.beta_1, opt.beta_2, opt.epsilon,
+                                   1, stream_ptr()), 'adam_dense')
+
+
+def capture_step(body, around=contextlib.nullcontext):
+    """Capture one train step, ``body(x)`` run inside ``with around() as x``, in a CUDA graph.  Its kernels must read the
+    step counter, the rates and any seeds from device memory.  Returns (graph, what body returned, launches of this
+    library in one replay), or None after a warning when capture fails here: the caller then runs eagerly."""
+    import gc
+    try:
+        gc.collect()             # no autograd graph of an earlier (eager) step may outlive into the capture
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        l0 = N.lib.dtb_launch_count()
+        with around() as x, torch.cuda.graph(graph):
+            out = body(x)
+        n_launch = N.lib.dtb_launch_count() - l0          # kernels of this library inside one replay
+    except Exception as exc:
+        import warnings
+        warnings.warn(f'deeptables_b200: CUDA-graph capture of the train step failed ({type(exc).__name__}: {exc}); '
+                      f'continuing with eager launches')
+        torch.cuda.synchronize()
+        return None
+    N.lib.dtb_launch_count_add(-n_launch)                # counted at capture, not executed yet
+    return graph, out, n_launch
 
 
 def _native_optim_params(spec):

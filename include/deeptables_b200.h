@@ -480,6 +480,21 @@ int dtb_gbdt_leaves(const int32_t* cat, int cat_stride, const float* cont, int c
 int dtb_discretize(const float* cont, int cont_stride, int64_t rows, const int32_t* src_col, const double* edges,
                    const int64_t* edge_off, int n_cols, int32_t* out_cat, int out_stride, int out_col, void* stream);
 
+/* ---- denoising auto-encoder batches (deeptables_b200/dae.py; reference fe/dae.py) ---------------------------------- */
+/* One training batch of rows <= batch_rows rows from X [*, cols] (float32, row-major), with
+ * base = (*step_dev - *epoch_first_step_dev) * batch_rows and s = *step_dev + 1 read from device memory, so that one
+ * captured CUDA graph serves every full batch of every epoch:
+ *   x_tgt[i, :] = X[p1[base + i], :]
+ *   x_in[i, c]  = X[p2[base + i], c] when c is one of row i's k swapped columns at step s, else x_tgt[i, c].
+ * The swapped columns of row i are the k columns c with the smallest keys (h << 32) | c, compared as unsigned 64-bit
+ * integers, where h is the 32-bit counter hash (mix32 of dtb_common.cuh, seed < 2^32, every operand taken mod 2^32)
+ *   a = mix32((seed << 32) | s),  b = mix32((a << 32) | i),  h = mix32((b << 32) | c).
+ * k == cols takes the donor row whole.  p2 and x_in are NULL exactly when k == 0 (x_in may also be given then: it gets
+ * x_tgt).  p1 / p2 entries are the caller's to keep inside X.  No host synchronisation. */
+int dtb_dae_swap_batch(const float* X, int cols, const int64_t* p1, const int64_t* p2, const int* step_dev,
+                       const int* epoch_first_step_dev, int batch_rows, int rows, int k, unsigned long long seed,
+                       float* x_in, float* x_tgt, void* stream);
+
 /* Data-parallel exchange of the embedding gradient by rows (deepmodel.py:88-103: MirroredStrategy
  * exchanges embedding gradients as IndexedSlices too).  pack: every (b,f) reference claims its row once
  * per step (claim[row] = step); the owner MOVES the accumulated gradient row into packed[b,f,:] and zeroes
