@@ -35,8 +35,8 @@ def state_of(plan, y, p):
         cnt[3 + 2 * cols:3 + 3 * cols] = (~pred & label).sum(0)
     for li, thresholds in enumerate(plan.lists):
         t = np.asarray(thresholds, np.float32)
-        with np.errstate(invalid='ignore'):
-            bucket = (t[None, None, :] < p[:, :, None]).sum(-1)         # thresholds strictly below p; NaN: none
+        # thresholds strictly below p (the list is ascending); NaN: none
+        bucket = np.where(np.isnan(p), 0, np.searchsorted(t, p, side='left'))
         hist = np.zeros((cols, 2, len(t) + 1), np.uint64)
         for c in range(cols):
             for lab in (0, 1):
