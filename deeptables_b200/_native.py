@@ -136,6 +136,7 @@ _SIGNATURES = {
     'dtb_importance_sums': (c_int, [c_int, P, P, P, c_int64, c_int, c_double, P, P, P]),
     'dtb_shap_compose': (c_int, [P, P, P, P, P, c_int, P, P, P, c_int64, c_int, c_int, c_int, P, P, P]),
     'dtb_shap_means': (c_int, [P, c_int64, c_int, c_int, c_int, P, P]),
+    'dtb_pdp_block_sums': (c_int, [P, P, c_int64, c_int, c_int, c_int, P, P]),
     'dtb_gbdt_bin': (c_int, [P, c_int, P, c_int, P, P, P, c_int64, c_int, P, P]),
     'dtb_gbdt_grad': (c_int, [P, P, c_int64, c_int, c_int, c_int, P, P, P, P]),
     'dtb_gbdt_fixed': (c_int, [P, P, c_int64, c_int, c_int, P, P, P]),

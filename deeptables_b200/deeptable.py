@@ -99,6 +99,7 @@ class DefaultPreprocessor:
         if len(set(X.columns)) != len(X.columns):
             raise ValueError('Columns with duplicate names in X.')
         X.columns = [str(c) for c in X.columns]
+        self.feature_names_in_ = list(X.columns)          # the fitted frame's columns, excluded ones included
         self.task_ = self._infer_task(y)
         y = np.asarray(y).reshape(-1)
         if self.task_ in (consts.TASK_BINARY, consts.TASK_MULTICLASS) and self.config.auto_encode_label:

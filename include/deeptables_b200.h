@@ -403,6 +403,15 @@ int dtb_shap_compose(const int32_t* x_cat, const float* x_cont, const int32_t* b
 int dtb_shap_means(const float* prob, int64_t groups, int rows_per_group, int cols, int kind, double* out,
                    void* stream);
 
+/* ---- partial dependence (deeptables_b200/utils/partial_dependence.py) --------------------------------------------- */
+/* prob [groups*rows_per_group, cols]: row k*rows_per_group + j is row j of group k.  The rows of each group are cut into
+ * blocks of block_rows (the last may be short); out [groups, blocks, cols] (float64) receives, for each block and
+ * column, the sum over its rows of weight[j] * prob (weight [rows_per_group] float64, or NULL for weight 1).  Each sum
+ * has one fixed order (lane stride 32 within the block, then a fixed butterfly), so a block's sum is the same bits
+ * wherever the block sits in a launch. */
+int dtb_pdp_block_sums(const float* prob, const double* weight, int64_t groups, int rows_per_group, int cols,
+                       int block_rows, double* out, void* stream);
+
 /* ---- gradient-boosted leaf features (deeptables_b200/gbm.py; reference preprocessor.py:431-452) ------------------- */
 /* Feature i of a booster is read from the model's own inputs: feat_col[i] = c >= 0 is column c of cat [rows, cat_stride]
  * (int32 codes, compared as their float32 values), feat_col[i] = -1 - c is column c of cont [rows, cont_stride].
