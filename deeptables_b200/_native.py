@@ -82,12 +82,14 @@ _SIGNATURES = {
     'dtb_embedding_scatter_add': (c_int, [P, P, P, P, c_int, c_int, c_int, P]),
     'dtb_fm_linear_fwd': (c_int, [P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, P, P]),
     'dtb_fm_linear_bwd': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
+    'dtb_linear_dense_grad': (c_int, [P, P, P, c_int, c_int, P]),
     'dtb_concat_emb_dense_fwd': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P, P]),
     'dtb_concat_emb_dense_bwd': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_ragged_concat_emb_dense_fwd': (c_int, [P, P, P, _IP, P, P, c_int, c_int, c_int, c_int, P, P]),
     'dtb_ragged_concat_emb_dense_bwd': (c_int, [P, P, _IP, P, P, c_int, c_int, c_int, c_int, P]),
     'dtb_batchnorm_train_fwd': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_float, c_float, P]),
     'dtb_batchnorm_infer_fwd': (c_int, [P, P, P, P, P, P, c_int, c_int, c_float, P]),
+    'dtb_batchnorm_infer_bwd': (c_int, [P, P, P, P, c_int, c_int, c_float, P]),
     'dtb_batchnorm_bwd': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_float, P]),
     'dtb_dense_workspace_bytes': (c_size_t, [c_int, c_int]),
     'dtb_dense_fwd': (c_int, [P, P, P, P, P, c_size_t, c_int, c_int, c_int, c_int, P]),
@@ -137,6 +139,10 @@ _SIGNATURES = {
     'dtb_shap_compose': (c_int, [P, P, P, P, P, c_int, P, P, P, c_int64, c_int, c_int, c_int, P, P, P]),
     'dtb_shap_means': (c_int, [P, c_int64, c_int, c_int, c_int, P, P]),
     'dtb_pdp_block_sums': (c_int, [P, P, c_int64, c_int, c_int, c_int, P, P]),
+    'dtb_gradshap_compose': (c_int, [P, P, P, P, P, P, P, c_int, P, P, P, c_int64, c_int, c_int, c_int, P, P, P]),
+    'dtb_gradshap_reduce': (c_int, [P, P, P, P, P, P, P, c_int, P, P, c_int64, c_int, c_int, P, P, P, P]),
+    'dtb_gradshap_means': (c_int, [P, c_int64, c_int, c_int, P, P]),
+    'dtb_gradshap_output_grad': (c_int, [P, c_int64, c_int, c_int, c_int, P, P]),
     'dtb_gbdt_bin': (c_int, [P, c_int, P, c_int, P, P, P, c_int64, c_int, P, P]),
     'dtb_gbdt_grad': (c_int, [P, P, c_int64, c_int, c_int, c_int, P, P, P, P]),
     'dtb_gbdt_fixed': (c_int, [P, P, c_int64, c_int, c_int, P, P, P]),

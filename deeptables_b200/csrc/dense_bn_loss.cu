@@ -102,6 +102,17 @@ __global__ void bn_apply_kernel(const float* __restrict__ X, float* __restrict__
   }
 }
 
+// dX = dY * (rsqrt(var + eps) * gamma): the factors of bn_apply_kernel's scale in its order
+__global__ void bn_infer_bwd_kernel(const float* __restrict__ dY, float* __restrict__ dX,
+                                    const float* __restrict__ gamma, const float* __restrict__ var, float eps,
+                                    int64_t total, int cols) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % cols);
+    dX[i] = dY[i] * (rsqrtf(var[c] + eps) * gamma[c]);
+  }
+}
+
 __global__ void bn_bwd_apply_kernel(const float* __restrict__ X, const float* __restrict__ dY,
                                     float* __restrict__ dX, const float* __restrict__ gamma,
                                     const float* __restrict__ mean, const float* __restrict__ var,
@@ -646,6 +657,17 @@ int dtb_batchnorm_infer_fwd(const float* X, float* Y, const float* gamma, const 
   return DTB_OK;
 }
 
+int dtb_batchnorm_infer_bwd(const float* dY, float* dX, const float* gamma, const float* moving_var, int rows,
+                            int cols, float eps, void* stream) {
+  DTB_CHECK_ARG(dY && dX && gamma && moving_var, "NULL argument");
+  DTB_CHECK_ARG(rows >= 0 && cols > 0, "bad shape");
+  const int64_t total = (int64_t)rows * cols;
+  if (total == 0) return DTB_OK;
+  bn_infer_bwd_kernel<<<ew_grid(total), 256, 0, (cudaStream_t)stream>>>(dY, dX, gamma, moving_var, eps, total, cols);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
+
 int dtb_batchnorm_bwd(const float* X, const float* dY, float* dX, const float* gamma, const float* save_mean,
                       const float* save_var, float* dgamma, float* dbeta, double* workspace, int rows,
                       int cols, float eps, void* stream) {
@@ -697,7 +719,8 @@ int dtb_dense_fwd(const float* X, const float* W, const float* bias, float* Y, v
 int dtb_dense_bwd(const float* X, const float* W, const float* Y, float* dY, float* dX, float* dW,
                   float* dbias, void* workspace, size_t workspace_bytes, int rows, int in_dim, int out_dim, int act,
                   void* stream) {
-  DTB_CHECK_ARG(X && W && dY && dW, "NULL argument");
+  DTB_CHECK_ARG(X && W && dY && (dW || dX), "NULL argument");
+  DTB_CHECK_ARG(dW || !dbias, "dbias without dW");
   DTB_CHECK_ARG(act == DTB_ACT_NONE || ((act == DTB_ACT_RELU || act == DTB_ACT_TANH) && Y), "relu / tanh backward needs Y");
   DTB_CHECK_ARG(rows >= 0 && in_dim > 0 && out_dim > 0, "bad shape");
   if (rows == 0) return DTB_OK;
@@ -715,10 +738,12 @@ int dtb_dense_bwd(const float* X, const float* W, const float* Y, float* dY, flo
       col_sum_float_kernel<<<grid, block, 0, st>>>(dY, dbias, rows, out_dim, rpb);
       DTB_LAUNCH_OK();
     }
-    col_reduce_grid(rows, in_dim, grid, block, rpb);
-    grid.z = out_dim;
-    dense_narrow_bwd_dw<<<grid, block, 0, st>>>(X, dY, dW, rows, in_dim, out_dim, rpb);
-    DTB_LAUNCH_OK();
+    if (dW) {
+      col_reduce_grid(rows, in_dim, grid, block, rpb);
+      grid.z = out_dim;
+      dense_narrow_bwd_dw<<<grid, block, 0, st>>>(X, dY, dW, rows, in_dim, out_dim, rpb);
+      DTB_LAUNCH_OK();
+    }
     if (dX) {
       const int64_t total_in = (int64_t)rows * in_dim;
       dense_narrow_bwd_dx<<<ew_grid(total_in), 256, 0, st>>>(dY, W, dX, total_in, in_dim, out_dim);
@@ -727,7 +752,8 @@ int dtb_dense_bwd(const float* X, const float* W, const float* Y, float* dY, flo
     return DTB_OK;
   }
   // dW[in,out] += X^T dZ and dbias += colsum(dZ) in one wgmma kernel; dX[rows,in] = dZ W^T in another
-  int rc = dense_tc_wgrad(X, in_dim, dY, out_dim, dW, out_dim, dbias, rows, in_dim, out_dim, st);
+  int rc = DTB_OK;
+  if (dW) rc = dense_tc_wgrad(X, in_dim, dY, out_dim, dW, out_dim, dbias, rows, in_dim, out_dim, st);
   if (rc != DTB_OK) return rc;
   if (dX)
     rc = dense_tc_rows(dY, out_dim, W, out_dim, 1, nullptr, dX, in_dim, rows, out_dim, in_dim, DTB_ACT_NONE, workspace,

@@ -432,11 +432,30 @@ static bool vec_ok(int D, const void* table) {
 }
 
 
+__global__ void linear_dense_grad_kernel(const float* __restrict__ g_lin, const float* __restrict__ w_dense,
+                                         float* __restrict__ d_dense, int64_t total, int C) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
+    d_dense[i] = g_lin[i / C] * w_dense[i % C];
+}
+
 }  // namespace dtb
 
 using namespace dtb;
 
 extern "C" {
+
+int dtb_linear_dense_grad(const float* g_lin, const float* w_dense, float* d_dense, int B, int C, void* stream) {
+  DTB_CHECK_ARG(g_lin && w_dense && d_dense, "NULL argument");
+  DTB_CHECK_ARG(B >= 0 && C > 0, "bad shape");
+  const int64_t total = (int64_t)B * C;
+  if (total == 0) return DTB_OK;
+  int blocks = ceil_div(total, 256);
+  const int cap = sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  linear_dense_grad_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(g_lin, w_dense, d_dense, total, C);
+  DTB_LAUNCH_OK();
+  return DTB_OK;
+}
 
 int dtb_fm_linear_fwd(const int32_t* idx, const float* table, const int64_t* row_offsets,
                       const float* dense, const float* w_lin, float* out_lin, float* out_fm, int B, int F,

@@ -174,6 +174,17 @@ class _Scope:
             self.buffers[name] = b
         return b
 
+    @contextlib.contextmanager
+    def fixed_params(self):
+        """Inside: every parameter the layers ask for is a detached view of itself, so a backward computes input
+        gradients only -- no weight-gradient kernel runs and nothing is added into the parameters' gradients."""
+        params = self.params
+        self.params = OrderedDict((n, p.detach()) for n, p in params.items())
+        try:
+            yield
+        finally:
+            self.params = params
+
     def flatten_embeddings(self, emb_list):
         mat = emb_list.block.materialize()
         return mat.reshape(mat.shape[0], -1)
@@ -406,8 +417,9 @@ class DeepModel:
         self.model = KerasLikeModel(self)
         return self.model
 
-    def _forward(self, cat, cont, training, describe=False, capture=None):
-        """inputs -> embeddings -> nets -> stacking -> task_output pre-activation z."""
+    def _forward(self, cat, cont, training, describe=False, capture=None, emb=None):
+        """inputs -> embeddings -> nets -> stacking -> task_output pre-activation z.  ``emb``: the field embeddings
+        themselves instead of ``cat``'s gather: (B, F, D) or, for fields of different widths, (B, sum D_i)."""
         cfg = self.config
         scope = self._scope
         scope.training = training
@@ -416,7 +428,11 @@ class DeepModel:
         with L.scope_guard(scope):
             embeddings = []
             block = None
-            if self.n_fields and self.table.ragged:
+            if self.n_fields and emb is not None:
+                block = E.RaggedFieldBlock(None, self.table, flat=emb) if self.table.ragged else \
+                    E.FieldBlock.from_tensor(emb)
+                embeddings = E.RaggedEmbeddingList(block) if self.table.ragged else E.EmbeddingList(block)
+            elif self.n_fields and self.table.ragged:
                 # fields of different widths: one flat (B, sum D_i) gather feeds flatten_embeddings, the list items
                 # (B, 1, D_i) and, with dropout, concat_embedding_dense, so they all share one mask
                 block = E.RaggedFieldBlock(cat, self.table)
@@ -811,6 +827,15 @@ class DeepModel:
     # ------------------------------------------------------------------------------------------
     # host <-> device input plumbing  (replaces utils/dataset_generator.py:36-72)
     # ------------------------------------------------------------------------------------------
+    def input_forward(self, emb, cont):
+        """The inference forward (no dropout, BatchNormalization on its moving statistics) of a materialised embedding
+        block ``emb`` -- (B, F, D), or (B, sum D_i) for fields of different widths -- and the continuous inputs
+        ``cont`` (B, C), with autograd recording: the pre-activation z [B, outputs], whose backward gives the
+        gradients of ``emb`` and ``cont`` only.  The parameters are held fixed (no weight gradient is computed or
+        accumulated) and the table, its gradient, the optimiser and the dropout seeds are not touched."""
+        with torch.enable_grad(), self._scope.fixed_params():
+            return self._forward(None, cont, training=False, emb=emb)
+
     def _to_device_inputs(self, X, device=None):
         """DataFrame / dict of arrays -> (cat int32 [N,F] | None, cont float32 [N,C] | None) on ``device`` (default: the GPU)."""
         device = self.device if device is None else device

@@ -333,7 +333,12 @@ class FMLinearFn(torch.autograd.Function):
         if t is not None:
             _table_grad_done(t)
         ga = _TableBackwardMixin.finish_tensor_table(t) if t is not None else None
-        return ga, None, gw, None, None, None
+        gd = None
+        if ctx.needs_input_grad[1] and want_lin:       # input gradients (explain.gradient_values); training never asks
+            gd = torch.empty_like(dense)
+            check(N.lib.dtb_linear_dense_grad(ptr(g_lin), ptr(w_lin[f:]), ptr(gd), b, c, stream_ptr()),
+                  'linear_dense_grad')
+        return ga, gd, gw, None, None, None
 
 
 class ConcatEmbDenseFn(torch.autograd.Function):
@@ -360,7 +365,8 @@ class ConcatEmbDenseFn(torch.autograd.Function):
         check(N.lib.dtb_concat_emb_dense_bwd(ptr(idx), ptr(offs), ptr(g), ptr(gt), b, f, d, c, stream_ptr()),
               'concat_emb_dense_bwd')
         _table_grad_done(t)
-        return _TableBackwardMixin.finish_tensor_table(t), None, None
+        gd = g[:, f * d:] if ctx.needs_input_grad[1] else None      # training never asks
+        return _TableBackwardMixin.finish_tensor_table(t), gd, None
 
 
 class RaggedConcatEmbDenseFn(torch.autograd.Function):
@@ -388,7 +394,8 @@ class RaggedConcatEmbDenseFn(torch.autograd.Function):
                                                     idx.shape[0], t.n_fields, t.dim, ctx.c, stream_ptr()),
               'ragged_concat_emb_dense_bwd')
         _table_grad_done(t)
-        return None, None, None
+        gd = g[:, sum(t.field_dims):] if ctx.needs_input_grad[1] else None      # training never asks
+        return None, gd, None
 
 
 class BatchNormFn(torch.autograd.Function):
@@ -433,6 +440,26 @@ def batchnorm_infer(x, gamma, beta, moving_mean, moving_var):
     check(N.lib.dtb_batchnorm_infer_fwd(ptr(x), ptr(y), ptr(gamma), ptr(beta), ptr(moving_mean),
                                         ptr(moving_var), rows, cols, BN_EPS, stream_ptr()), 'batchnorm_infer_fwd')
     return y
+
+
+class BatchNormInferFn(torch.autograd.Function):
+    """keras BatchNormalization in inference (the moving statistics), differentiated with respect to its input only:
+    the input gradient with the parameters and statistics held fixed (explain.gradient_values)."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, moving_mean, moving_var):
+        ctx.save_for_backward(gamma, moving_var)
+        return batchnorm_infer(x, gamma, beta, moving_mean, moving_var)
+
+    @staticmethod
+    def backward(ctx, dy):
+        gamma, moving_var = ctx.saved_tensors
+        dy = _f32(dy)
+        cols = dy.shape[-1]
+        dx = torch.empty_like(dy)
+        check(N.lib.dtb_batchnorm_infer_bwd(ptr(dy), ptr(dx), ptr(gamma), ptr(moving_var), dy.numel() // cols, cols,
+                                            BN_EPS, stream_ptr()), 'batchnorm_infer_bwd')
+        return dx, None, None, None, None
 
 
 def _seed_args(seed):
@@ -502,8 +529,10 @@ class DenseFn(torch.autograd.Function):
         if ctx.act:
             dz = dz.clone()                             # overwritten with d(pre-activation)
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        dw = torch.zeros_like(kernel)
-        db = torch.zeros(out_dim, dtype=torch.float32, device=x.device) if ctx.has_bias else None
+        # input gradients with the weights held fixed (explain.gradient_values) skip the weight-gradient kernels
+        want_w = ctx.needs_input_grad[1]
+        dw = torch.zeros_like(kernel) if want_w else None
+        db = torch.zeros(out_dim, dtype=torch.float32, device=x.device) if ctx.has_bias and want_w else None
         ws_bytes = N.lib.dtb_dense_workspace_bytes(in_dim, out_dim)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device) if ws_bytes else None
         check(N.lib.dtb_dense_bwd(ptr(x), ptr(kernel), ptr(y), ptr(dz), ptr(dx), ptr(dw), ptr(db), ptr(ws), ws_bytes,
@@ -545,17 +574,20 @@ class CINFn(torch.autograd.Function):
         sizes_c = N.int_array(sizes)
         g = _f32(g)
         gt = _grad_target(t)
-        dw = torch.zeros_like(weights)
-        db = torch.zeros(sum(sizes), dtype=torch.float32, device=w.device) if ctx.has_bias else None
+        want_w = ctx.needs_input_grad[1]       # False for input gradients with the weights held fixed
+        dw = torch.zeros_like(weights) if want_w else torch.empty_like(weights)
+        db = torch.zeros(sum(sizes), dtype=torch.float32, device=w.device) if ctx.has_bias and want_w else None
         args = (ptr(idx), ptr(w), ptr(offs), ptr(weights), ptr(g), ptr(ctx.saved_buf), ptr(gt), ptr(dw), ptr(db),
                 ptr(ctx.ws), ctx.ws.numel(), b, f, d, sizes_c, len(sizes), direct, act, precision)
         # phase 1: everything that adds into the table gradient; then (data parallel) the exchange of the
         # table gradient may start and overlap phase 2, the weight-gradient kernels
         check(N.lib.dtb_cin_bwd_phase(*args, 1, stream_ptr()), 'cin_bwd(dgrad)')
         _table_grad_done(t)
-        check(N.lib.dtb_cin_bwd_phase(*args, 2, stream_ptr()), 'cin_bwd(wgrad)')
+        if want_w:
+            check(N.lib.dtb_cin_bwd_phase(*args, 2, stream_ptr()), 'cin_bwd(wgrad)')
         ctx.saved_buf = ctx.ws = None
-        return (_TableBackwardMixin.finish_tensor_table(t), dw, db, None, None, None, None, None, None)
+        return (_TableBackwardMixin.finish_tensor_table(t), dw if want_w else None, db, None, None, None, None, None,
+                None)
 
 
 class CrossFn(torch.autograd.Function):

@@ -349,3 +349,175 @@ def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, t
         torch.cuda.synchronize()
         stages.update(timer.result())
     return phi
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# expected gradients (utils.shap.DeepTablesGradientExplainer)
+# ---------------------------------------------------------------------------------------------------------------------
+GRAD_IDENTITY, GRAD_SIGMOID, GRAD_SOFTMAX = 0, 1, 2      # DTB_GRADSHAP_* (deeptables_b200.h)
+_ALPHA_BITS = 24                                          # alpha is a multiple of 2^-24: exact in float32, below 1
+
+
+def check_gradient_options(dt_model):
+    """The derived columns of ``apply_gbm_features`` and ``auto_discrete`` are step functions of the continuous inputs:
+    a gradient cannot attribute their jumps."""
+    cfg = getattr(dt_model, 'config', None)
+    for option in ('apply_gbm_features', 'auto_discrete'):
+        if cfg is not None and getattr(cfg, option, False):
+            raise NotImplementedError(f'{option}=True: expected gradients cannot attribute the jumps of its derived '
+                                      f'columns')
+
+
+def check_positive_int(value, name):
+    if isinstance(value, bool) or not isinstance(value, numbers.Integral) or value < 1:
+        raise ValueError(f'{name} must be a positive integer, got {value!r}')
+
+
+def gradient_draws(seed, i, nsamples, bg_rows, rng=None):
+    """The samples of explained row i: background rows j (int32 [nsamples], uniform with replacement) then the
+    interpolation points alpha (float32 [nsamples], uniform on [0, 1) in steps of 2^-24), both from
+    ``np.random.RandomState([seed, i])``.  ``rng``: a RandomState to reseed instead of building one (the same draws,
+    at a sixth of the host time)."""
+    if rng is None:
+        rng = np.random.RandomState()
+    rng.seed([seed, i])
+    j = rng.randint(0, bg_rows, size=nsamples).astype(np.int32)
+    alpha = (np.floor(rng.random_sample(nsamples) * 2.0 ** _ALPHA_BITS) / 2.0 ** _ALPHA_BITS).astype(np.float32)
+    return j, alpha
+
+
+def output_kind(task):
+    return {consts.TASK_REGRESSION: GRAD_IDENTITY, consts.TASK_MULTICLASS: GRAD_SOFTMAX}.get(task, GRAD_SIGMOID)
+
+
+def output_means(bg, cat, cont, rows, batch_size):
+    """float64 [outputs]: the mean of the explained output (the output layer) over ``rows`` input rows."""
+    pred = torch.empty(rows, bg.cols, dtype=torch.float32, device=bg.model.device)
+    forward_rows(bg.model, cat, cont, pred, batch_size)
+    return pred.cpu().numpy().astype(np.float64).mean(axis=0)
+
+
+class _Embeddings:
+    """What the gradient kernels read of the model's embedding table: the table, its row offsets and the column offset
+    of each field in a flat row (device int32 [F + 1])."""
+
+    def __init__(self, model):
+        t = model.table
+        self.table, self.row_offsets, self.dim, self.ragged = t.weight, t.row_offsets, t.dim, t.ragged
+        self.fields = t.n_fields
+        self.col_offsets = torch.tensor(np.concatenate([[0], np.cumsum(t.field_dims)]), dtype=torch.int32,
+                                        device=model.device)
+        self.width = int(sum(t.field_dims))
+
+
+def gradient_values(bg, X, nsamples=200, seed=0, batch_size=65536, stages=None):
+    """float64 [len(X), columns, outputs] expected gradients of the output layer at each row of X against ``bg``.
+
+    Pair (i, s) interpolates between row i and background row j_s at alpha_s (``gradient_draws``); its value in an
+    encoded column is the gradient of the output there times the column's difference x - b (summed over the
+    embedding coordinates of a categorical field); a row's value is the mean over its samples.  Each frame column
+    takes the value of the encoded column read from it, 0 when the model reads none.  ``stages``: a dict that receives
+    the seconds spent in compose, forward, backward, reduce and means (CUDA events) and on the host in encode (the
+    preprocessor and the upload) and draws."""
+    check_positive_int(nsamples, 'nsamples')
+    check_positive_int(batch_size, 'batch_size')
+    if X.columns.to_list() != bg.columns:
+        raise ValueError(f'X has columns {X.columns.to_list()}, the explainer {bg.columns}')
+    model, dev = bg.model, bg.model.device
+    n_rows, n_cols, K, N_bg = len(X), len(bg.columns), bg.cols, bg.rows
+    phi = np.zeros((n_rows, n_cols, K), np.float64)
+    if n_rows == 0:
+        return phi
+    timer = _Stages() if stages is not None else None
+    model.flush_optimizer_state()
+    t0 = time.perf_counter()
+    x_cat, x_cont = bg.encode(X)
+    if timer:
+        timer.host['encode'] += time.perf_counter() - t0
+    F = x_cat.shape[1] if x_cat is not None else 0
+    C = x_cont.shape[1] if x_cont is not None else 0
+    emb = _Embeddings(model) if F else None
+    kind = output_kind(model.task)
+    bits = np.concatenate([bg.cat_bit.cpu().numpy(), bg.cont_bit.cpu().numpy()])     # frame column of each encoded one
+    cols = F + C
+
+    rank, world = (torch.distributed.get_rank(), dp.world_size()) if dp.is_distributed() else (0, 1)
+    mine = list(range(rank, n_rows, world))
+    group_rows = max(1, batch_size // nsamples)
+    rng = np.random.RandomState()
+
+    def event(name, end=None):
+        if end is not None:
+            end.record()
+        return timer.device(name) if timer and name else None
+
+    def tables():
+        return (ptr(x_cat), ptr(x_cont), ptr(bg.cat), ptr(bg.cont), ptr(emb.table) if F else None,
+                ptr(emb.row_offsets) if F else None, ptr(emb.col_offsets) if F else None, emb.dim if F else 0)
+
+    for g0 in range(0, len(mine), group_rows):
+        group = mine[g0:g0 + group_rows]
+        t0 = time.perf_counter()
+        draws = [gradient_draws(seed, i, nsamples, N_bg, rng) for i in group]
+        if timer:
+            timer.host['draws'] += time.perf_counter() - t0
+        x_index = torch.as_tensor(np.repeat(np.array(group, np.int32), nsamples)).to(dev)
+        bg_index = torch.as_tensor(np.concatenate([d[0] for d in draws])).to(dev)
+        alpha = torch.as_tensor(np.concatenate([d[1] for d in draws])).to(dev)
+        P = len(group) * nsamples
+        values = torch.empty(K, P, cols, dtype=torch.float64, device=dev)
+        for p0 in range(0, P, batch_size):
+            m = min(batch_size, P - p0)
+            end = event('compose')
+            out_emb = torch.empty((F, m, emb.dim) if not emb.ragged else (m, emb.width), dtype=torch.float32,
+                                  device=dev) if F else None
+            out_cont = torch.empty(m, C, dtype=torch.float32, device=dev) if C else None
+            check(N.lib.dtb_gradshap_compose(*tables(), ptr(x_index[p0:]), ptr(bg_index[p0:]), ptr(alpha[p0:]), m, F,
+                                             C, 0 if F and emb.ragged else 1, ptr(out_emb), ptr(out_cont),
+                                             stream_ptr()), 'gradshap_compose')
+            inputs = []
+            if F:       # the tensor-backed field block reads [F, m, D] in place; its gradient comes back as (m, F, D)
+                out_emb = (out_emb if emb.ragged else out_emb.permute(1, 0, 2)).detach().requires_grad_(True)
+                inputs.append(out_emb)
+            if C:
+                out_cont = out_cont.requires_grad_(True)
+                inputs.append(out_cont)
+            end = event('forward', end)
+            z = model.input_forward(out_emb, out_cont)
+            end = event(None, end)
+            dz = torch.empty(m, K, dtype=torch.float32, device=dev)
+            for k in range(K):
+                end = event('backward')
+                check(N.lib.dtb_gradshap_output_grad(ptr(z.detach()), m, K, k, kind, ptr(dz), stream_ptr()),
+                          'gradshap_output_grad')
+                grads = torch.autograd.grad(z, inputs, grad_outputs=dz, retain_graph=k < K - 1, allow_unused=True)
+                grads = [torch.zeros_like(t) if g is None else g.contiguous() for t, g in zip(inputs, grads)]
+                g_emb = grads[0] if F else None
+                g_cont = grads[-1] if C else None
+                end = event('reduce', end)
+                check(N.lib.dtb_gradshap_reduce(*tables(), ptr(x_index[p0:]), ptr(bg_index[p0:]), m, F, C,
+                                                ptr(g_emb), ptr(g_cont), ptr(values[k, p0:]), stream_ptr()),
+                      'gradshap_reduce')
+                event(None, end)
+            del z, inputs
+        end = event('means')
+        means = torch.empty(K, len(group), cols, dtype=torch.float64, device=dev)
+        for k in range(K):
+            check(N.lib.dtb_gradshap_means(ptr(values[k]), len(group), nsamples, cols, ptr(means[k]), stream_ptr()),
+                  'gradshap_means')
+        event(None, end)
+        host = means.cpu().numpy()
+        rows = np.array(group)
+        for e in range(cols):
+            if bits[e] >= 0:
+                phi[rows, bits[e], :] += host[:, :, e].T
+
+    if world > 1:
+        gathered = [None] * world
+        torch.distributed.all_gather_object(gathered, phi[mine])
+        for r in range(world):
+            phi[r::world] = gathered[r]
+    if stages is not None:
+        torch.cuda.synchronize()
+        stages.update(timer.result())
+    return phi

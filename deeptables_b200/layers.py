@@ -146,6 +146,8 @@ class BatchNormalization(Layer):
         mv = scope.buffer(f'{self.name}/moving_variance', (width,), 1.0)
         if scope.training:
             return E.BatchNormFn.apply(x, gamma, beta, mm, mv)
+        if torch.is_grad_enabled() and x.requires_grad:
+            return E.BatchNormInferFn.apply(x, gamma, beta, mm, mv)
         return E.batchnorm_infer(x, gamma, beta, mm, mv)
 
 
@@ -285,10 +287,12 @@ class CIN(Layer):
             bs = [scope.param(f'{self.name}/bias{i}', (size,), 'zeros')
                   for i, size in enumerate(self.cross_layer_size)]
             bias = torch.cat(bs) if len(bs) > 1 else bs[0]
-        pooled = E.CINFn.apply(block.table.anchor, weights.contiguous(), bias, block,
+        # the activations are saved whenever a backward will run: a train step, or input gradients in inference
+        weights = weights.contiguous()
+        backward = torch.is_grad_enabled() and (block.table.anchor.requires_grad or weights.requires_grad)
+        pooled = E.CINFn.apply(block.table.anchor, weights, bias, block,
                                tuple(self.cross_layer_size), bool(self.direct),
-                               E.ACT_CODES[self.activation], int(self.precision),
-                               bool(scope.training and torch.is_grad_enabled()))
+                               E.ACT_CODES[self.activation], int(self.precision), bool(backward))
         with scope.name_prefix(self.name):
             if self.use_residual:
                 out0 = Dense(self.cross_layer_size[-1], activation=self.activation,

@@ -72,6 +72,9 @@ int dtb_fm_linear_fwd(const int32_t* idx, const float* table, const int64_t* row
 int dtb_fm_linear_bwd(const int32_t* idx, const float* table, const int64_t* row_offsets,
                       const float* dense, const float* w_lin, const float* g_lin, const float* g_fm,
                       float* grad_table, float* grad_wlin, int B, int F, int D, int C, void* stream);
+/* d_dense[B, C] = g_lin[b] * w_dense[c]: the gradient of the linear logit with respect to its continuous inputs
+ * (w_dense = w_lin + F, the weights of the continuous columns). */
+int dtb_linear_dense_grad(const float* g_lin, const float* w_dense, float* d_dense, int B, int C, void* stream);
 
 /* ---- flatten_embeddings + concat_embedding_dense (deepmodel.py:269-278,348-357) --------- */
 /* X[b, :] = [e[b,0,:], ..., e[b,F-1,:], dense[b,:]]   width W = F*D + C. */
@@ -104,6 +107,10 @@ int dtb_batchnorm_train_fwd(const float* X, float* Y, const float* gamma, const 
 int dtb_batchnorm_infer_fwd(const float* X, float* Y, const float* gamma, const float* beta,
                             const float* moving_mean, const float* moving_var, int rows, int cols,
                             float eps, void* stream);
+/* Backward of the inference forward with respect to X only: dX = dY * gamma / sqrt(moving_var + eps), the scale
+ * rounded as the forward rounds it.  dX may alias dY. */
+int dtb_batchnorm_infer_bwd(const float* dY, float* dX, const float* gamma, const float* moving_var, int rows,
+                            int cols, float eps, void* stream);
 /* Backward of the training forward.  dX may alias dY.  dgamma/dbeta [cols] accumulate. */
 int dtb_batchnorm_bwd(const float* X, const float* dY, float* dX, const float* gamma,
                       const float* save_mean, const float* save_var, float* dgamma, float* dbeta,
@@ -120,7 +127,8 @@ size_t dtb_dense_workspace_bytes(int in_dim, int out_dim);
 int dtb_dense_fwd(const float* X, const float* W, const float* bias, float* Y, void* workspace,
                   size_t workspace_bytes, int rows, int in_dim, int out_dim, int act, void* stream);
 /* dY holds dLoss/dY on entry and is overwritten with dLoss/d(pre-activation).  dX may be NULL.
- * dW[in,out] and dbias[out] accumulate (dbias may be NULL). */
+ * dW[in,out] and dbias[out] accumulate (dbias may be NULL).  dW NULL (then dbias must be NULL too, and dX set): no
+ * weight-gradient kernel runs. */
 int dtb_dense_bwd(const float* X, const float* W, const float* Y, float* dY, float* dX, float* dW,
                   float* dbias, void* workspace, size_t workspace_bytes, int rows, int in_dim, int out_dim,
                   int act, void* stream);
@@ -402,6 +410,35 @@ int dtb_shap_compose(const int32_t* x_cat, const float* x_cont, const int32_t* b
 #define DTB_SHAP_CLASS 1
 int dtb_shap_means(const float* prob, int64_t groups, int rows_per_group, int cols, int kind, double* out,
                    void* stream);
+
+/* ---- expected gradients (deeptables_b200/explain.py, utils/shap.py DeepTablesGradientExplainer) -------------------- */
+/* Pair p interpolates between explained row x_index[p] (x_cat [*, fields], x_cont [*, conts]) and background row
+ * bg_index[p] (bg_cat, bg_cont) at alpha[p]: every value is v = b + alpha * (x - b), each operation rounded on its own
+ * (no fused multiply-add).  Categorical field f interpolates its embedding rows (table [*, table_dim], row_offsets
+ * [fields+1]; an id out of range reads as zeros) over its first col_offsets[f+1] - col_offsets[f] coordinates.
+ * out_emb is [fields, pairs, table_dim] when field_major (every field of width table_dim: the layout of a tensor-backed
+ * field block) and [pairs, col_offsets[fields]] otherwise; out_cont is [pairs, conts].  fields or conts may be 0 (then
+ * their pointers may be NULL). */
+int dtb_gradshap_compose(const int32_t* x_cat, const float* x_cont, const int32_t* bg_cat, const float* bg_cont,
+                         const float* table, const int64_t* row_offsets, const int32_t* col_offsets, int table_dim,
+                         const int32_t* x_index, const int32_t* bg_index, const float* alpha, int64_t pairs,
+                         int fields, int conts, int field_major, float* out_emb, float* out_cont, void* stream);
+/* out [pairs, fields + conts] (float64): for field f, sum over d in order of g_emb[p, col_offsets[f] + d] times the
+ * float32 difference of the two embedding coordinates (g_emb [pairs, col_offsets[fields]]); for continuous column c,
+ * g_cont[p, c] times x - b.  A zero difference contributes exactly 0.  Arguments as dtb_gradshap_compose. */
+int dtb_gradshap_reduce(const int32_t* x_cat, const float* x_cont, const int32_t* bg_cat, const float* bg_cont,
+                        const float* table, const int64_t* row_offsets, const int32_t* col_offsets, int table_dim,
+                        const int32_t* x_index, const int32_t* bg_index, int64_t pairs, int fields, int conts,
+                        const float* g_emb, const float* g_cont, double* out, void* stream);
+/* out [rows, cols] (float64) = the mean of values [rows * samples, cols] over each row's samples, added in sample
+ * order. */
+int dtb_gradshap_means(const double* values, int64_t rows, int samples, int cols, double* out, void* stream);
+/* dz [rows, cols] = the derivative of output column k with respect to the pre-activation z [rows, cols]: the identity
+ * (regression), the sigmoid of each column (binary, multilabel) or the softmax over the columns (multiclass). */
+#define DTB_GRADSHAP_IDENTITY 0
+#define DTB_GRADSHAP_SIGMOID 1
+#define DTB_GRADSHAP_SOFTMAX 2
+int dtb_gradshap_output_grad(const float* z, int64_t rows, int cols, int k, int kind, float* dz, void* stream);
 
 /* ---- partial dependence (deeptables_b200/utils/partial_dependence.py) --------------------------------------------- */
 /* prob [groups*rows_per_group, cols]: row k*rows_per_group + j is row j of group k.  The rows of each group are cut into
