@@ -143,7 +143,14 @@ _SIGNATURES = {
     'dtb_gradshap_reduce': (c_int, [P, P, P, P, P, P, P, c_int, P, P, c_int64, c_int, c_int, P, P, P, P]),
     'dtb_gradshap_means': (c_int, [P, c_int64, c_int, c_int, P, P]),
     'dtb_gradshap_output_grad': (c_int, [P, c_int64, c_int, c_int, c_int, P, P]),
-    'dtb_gbdt_bin': (c_int, [P, c_int, P, c_int, P, P, P, c_int64, c_int, P, P]),
+    'dtb_te_remap': (c_int, [P, P, c_int64, c_int, P, P]),
+    'dtb_te_keys': (c_int, [P, P, P, c_int64, c_int, c_int, c_int, P, P]),
+    'dtb_te_segment_starts': (c_int, [P, c_int64, c_int64, P, P]),
+    'dtb_te_segment_stats': (c_int, [P, P, P, P, P, c_int64, c_int, P, P]),
+    'dtb_te_segment_join': (c_int, [P, P, c_int64, P, P]),
+    'dtb_te_encodings': (c_int, [P, P, P, P, P, P, c_int64, c_int, c_int, c_int, c_double, P, P, P]),
+    'dtb_te_gather': (c_int, [P, P, P, P, P, P, c_int64, c_int, c_int, c_int, c_int, P, P]),
+    'dtb_gbdt_bin':(c_int, [P, c_int, P, c_int, P, P, P, c_int64, c_int, P, P]),
     'dtb_gbdt_grad': (c_int, [P, P, c_int64, c_int, c_int, c_int, P, P, P, P]),
     'dtb_gbdt_fixed': (c_int, [P, P, c_int64, c_int, c_int, P, P, P]),
     'dtb_gbdt_hist': (c_int, [P, P, c_int64, c_int64, P, P, c_int, c_int, P, P, P, P]),

@@ -449,6 +449,54 @@ int dtb_gradshap_output_grad(const float* z, int64_t rows, int cols, int k, int 
 int dtb_pdp_block_sums(const float* prob, const double* weight, int64_t groups, int rows_per_group, int cols,
                        int block_rows, double* out, void* stream);
 
+/* ---- target encoding (deeptables_b200/target_encoding.py; reference preprocessing/utils.py) ---------------------- */
+/* A column's rows carry a category code (-1: unknown), a fold id in [0, folds) and, for class targets, a class index
+ * in [0, classes).  A continuous target has classes = 0.  Group g of a column's statistics is every fold (g = 0) or,
+ * when folds > 1, every fold but f (g = 1 + f): the fitting rows of the rows held out in fold f. */
+#define DTB_TE_CHUNK 1024
+#define DTB_TE_SMOOTH 0   /* scikit-learn, float smooth: (smooth mu + S) / (smooth + n); mu when smooth + n = 0 */
+#define DTB_TE_AUTO 1     /* scikit-learn, smooth='auto': l = var n / (var n + SSD / n); l (S / n) + (1 - l) mu, mu
+                             when l is NaN.  var is the group's target variance, SSD the category's sum of squared
+                             differences from S / n */
+#define DTB_TE_RECALLED 2 /* category_encoders' TargetEncoder as recalled, min_samples_leaf = 20:
+                             s = 1 / (1 + exp(-(n - 20) / smooth)); mu (1 - s) + (S / n) s; mu when n = 0 */
+/* out[i] = map[in[i]] when 0 <= in[i] < map_len, else -1 (the host's factorised codes into sorted category order). */
+int dtb_te_remap(const int64_t* in, const int32_t* map, int64_t n, int map_len, int32_t* out, void* stream);
+/* keys[i] = (code * folds + fold) * max(classes, 1) + class, where a code -1 counts as unknown_code; -1 when that is
+ * -1 too (the row joins no category).  codes NULL: every code is 0; fold NULL: every fold is 0; cls is read only when
+ * classes > 0.  scikit-learn counts the rows outside given categories toward the first one: unknown_code 0. */
+int dtb_te_keys(const int32_t* codes, const uint8_t* fold, const int32_t* cls, int64_t n, int folds, int classes,
+                int unknown_code, int64_t* keys, void* stream);
+/* keys [n] sorted ascending, each -1 or in [0, slots): starts[s] (s in [0, slots]) = the first position whose key is
+ * >= s (n for s = slots), so slot s holds starts[s+1] - starts[s] rows. */
+int dtb_te_segment_starts(const int64_t* keys, int64_t n, int64_t slots, int64_t* starts, void* stream);
+/* For each chunk of a slot's sorted rows (DTB_TE_CHUNK rows counted from the slot's start, the last may be short)
+ * beginning at position q: partial[q] = the sum over its rows r of y[perm[r]] (seg_sum NULL), or of (y[perm[r]] - c)^2
+ * with c = seg_sum[slot] / (the slot's rows).  Lane l of a warp adds rows q+l, q+l+32, ... in order, then a fixed
+ * butterfly; tile_rows (a multiple of 32) only splits the work between CTAs.  Other entries of partial are untouched. */
+int dtb_te_segment_stats(const int64_t* keys, const int64_t* perm, const double* y, const int64_t* starts,
+                         const double* seg_sum, int64_t n, int tile_rows, double* partial, void* stream);
+/* out[s] = the chunk partials of slot s added in chunk order (0 for an empty slot). */
+int dtb_te_segment_join(const int64_t* starts, const double* partial, int64_t slots, double* out, void* stream);
+/* table [groups, cats, n_out] and, when prior is not NULL, prior [groups, n_out] (float64), groups = folds + 1 when
+ * folds > 1, else 1; n_out = classes when classes > 2, else 1.  starts (and, for a continuous target, sums and m2: the
+ * joined chunk sums and sums of squares around each slot's mean) are one column's statistics keyed as dtb_te_keys; the
+ * p_ arrays are those of the whole target, keyed with every code 0.  For group g and output j, n, S are the rows and the
+ * target sum (class targets: the rows of class j, or of class 1 when classes = 2) over the group's folds, each added in
+ * increasing fold order, and mu the same ratio for the whole target.  Class targets take SSD and var in closed form from
+ * the counts; continuous ones add, in fold order, each fold's sum of squares plus n_k (mean_k - mean)^2.  The encoding
+ * is the formula DTB_TE_*. */
+int dtb_te_encodings(const int64_t* starts, const double* sums, const double* m2, const int64_t* p_starts,
+                     const double* p_sums, const double* p_m2, int64_t cats, int folds, int classes, int formula,
+                     double smooth, double* table, double* prior, void* stream);
+/* out[r * out_stride + c * n_out + j] (float64) = the encoding of codes[c * n + r] in group g (fold NULL: 0, else
+ * 1 + fold[r]) of column c, whose table [groups, cats[c], n_out] starts at table + table_off[c]; for code -1
+ * prior[g, j], or prior[unknown_group, j] when unknown_group >= 0 (scikit-learn's fit_transform gives every unknown
+ * row the last fold's mean); NaN for a code >= cats[c]. */
+int dtb_te_gather(const int32_t* codes, const uint8_t* fold, const double* table, const int64_t* table_off,
+                  const int32_t* cats, const double* prior, int64_t n, int cols, int n_out, int unknown_group,
+                  int out_stride, double* out, void* stream);
+
 /* ---- gradient-boosted leaf features (deeptables_b200/gbm.py; reference preprocessor.py:431-452) ------------------- */
 /* Feature i of a booster is read from the model's own inputs: feat_col[i] = c >= 0 is column c of cat [rows, cat_stride]
  * (int32 codes, compared as their float32 values), feat_col[i] = -1 - c is column c of cont [rows, cont_stride].
