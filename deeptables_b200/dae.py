@@ -21,9 +21,10 @@ from collections import OrderedDict
 import numpy as np
 import torch
 
-from . import callbacks as CB, consts, deepmodel as DM, engine as E, importance, layers as L, optimizers as O
+from . import callbacks as CB, consts, deepmodel as DM, engine as E, layers as L, optimizers as O
 from . import _native as N
 from ._native import check, ptr, stream_ptr
+from .analysis import draw_seed
 
 _DEFAULT_OPTIMIZER = O.Adam(learning_rate=0.001)
 
@@ -275,7 +276,7 @@ class DAE:
         plan = layer_plan(units, self.feature_units, self.activate, cols)
         L.Dense(1, activation=self.activate)         # NotImplementedError, before any device work, for what Dense lacks
         spec = O.resolve(self.optimizer)
-        seed = importance.draw_seed(self.random_state)
+        seed = draw_seed(self.random_state)
         return AutoEncoder(plan, self.kernel_initializer, spec, seed, torch.device('cuda', torch.cuda.current_device()))
 
     def build_dae(self, X):

@@ -19,16 +19,16 @@ any batch size or number of ranks.  Data parallel: every rank calls with the sam
 """
 import collections
 import itertools
-import numbers
 import time
 from math import comb
 
 import numpy as np
 import torch
 
-from . import _native as N, consts, discrete, dp
+from . import _native as N, consts, discrete
 from ._native import check, ptr, stream_ptr
-from .importance import forward_rows
+from .analysis import Stages, check_positive_int, fitted_model, forward_rows, gather_strided, is_int, model_columns, \
+    rank_share
 
 SHAP_VALUE, SHAP_CLASS = 0, 1             # DTB_SHAP_* (deeptables_b200.h)
 _NUMBER_TYPES = (int, float, np.number)
@@ -47,7 +47,7 @@ def budget(M, nsamples):
 def check_nsamples(nsamples):
     if isinstance(nsamples, str) and nsamples == 'auto':
         return
-    if isinstance(nsamples, bool) or not isinstance(nsamples, numbers.Integral) or nsamples < 1:
+    if not is_int(nsamples) or nsamples < 1:
         raise ValueError(f"nsamples must be 'auto' or a positive integer, got {nsamples!r}")
 
 
@@ -168,9 +168,7 @@ class Background:
     """The background rows, encoded and uploaded once, and E, the mean of the model function over them."""
 
     def __init__(self, dt_model, frame, batch_size):
-        model = dt_model.get_model() if dt_model is not None else None
-        if model is None or getattr(model, 'model', None) is None or isinstance(model, list):
-            raise ValueError('the DeepTable has no fitted model')
+        model = fitted_model(dt_model)
         if len(frame) < 1:
             raise ValueError('the background has no rows')
         self.dt_model, self.model = dt_model, model
@@ -181,8 +179,7 @@ class Background:
         self.kind = SHAP_VALUE if model.task == consts.TASK_REGRESSION else SHAP_CLASS
         model.flush_optimizer_state()           # every embedding row current: the forward needs no per-batch catch-up
         self.cat, self.cont = self.encode(frame)
-        cat_names = [c.name for c in model.categorical_columns]
-        cont_names = [name for c in model.continuous_columns for name in c.column_names]
+        cat_names, cont_names = model_columns(model)
         pos = {str(c): j for j, c in enumerate(self.columns)}
         dev = model.device
         # the bit of each encoded column in a coalition mask is its column's position in the frame
@@ -204,26 +201,6 @@ class Background:
         return out
 
 
-class _Stages:
-    """Seconds spent per stage: host clocks for host work, CUDA events for device work (read at the end)."""
-
-    def __init__(self):
-        self.host = collections.defaultdict(float)
-        self.events = collections.defaultdict(list)
-
-    def device(self, name):
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        self.events[name].append((start, end))
-        return end
-
-    def result(self):
-        out = dict(self.host)
-        for name, pairs in self.events.items():
-            out[name] = sum(s.elapsed_time(e) for s, e in pairs) / 1e3
-        return out
-
-
 def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, trace=None):
     """float64 [len(X), columns] Kernel SHAP values of the model function at each row of X against ``bg``.
 
@@ -231,23 +208,21 @@ def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, t
     stages timed with CUDA events).  ``trace``: a dict that receives, per explained row, its Row(varying columns,
     masks, weights, coalition values, f(x))."""
     check_nsamples(nsamples)
-    if isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral) or batch_size < 1:
-        raise ValueError(f'batch_size must be a positive integer, got {batch_size!r}')
+    check_positive_int(batch_size, 'batch_size')
     if X.columns.to_list() != bg.columns:
         raise ValueError(f'X has columns {X.columns.to_list()}, the explainer {bg.columns}')
     model, dev = bg.model, bg.model.device
     n_rows, n_cols, N_bg = len(X), len(bg.columns), bg.rows
     if n_rows == 0:
         return np.zeros((0, n_cols), np.float64)
-    timer = _Stages() if stages is not None else None
+    timer = Stages(stages)
     model.flush_optimizer_state()
     x_cat, x_cont = bg.encode(X)
     fx = bg.means(x_cat, x_cont, n_rows, 1, batch_size).cpu().numpy()
     x_values = X.to_numpy(dtype=object)
     phi = np.zeros((n_rows, n_cols), np.float64)
 
-    rank, world = (torch.distributed.get_rank(), dp.world_size()) if dp.is_distributed() else (0, 1)
-    mine = list(range(rank, n_rows, world))
+    mine = rank_share(n_rows)
     per_chunk = max(1, batch_size // N_bg)          # coalitions per compose launch
     F = x_cat.shape[1] if x_cat is not None else 0
     C = x_cont.shape[1] if x_cont is not None else 0
@@ -274,8 +249,7 @@ def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, t
                 m[:, vary] = masks
                 full.append(m)
                 x_index.append(np.full(len(m), i, np.int32))
-        if timer:
-            timer.host['sampling'] += time.perf_counter() - t0
+        timer.host('sampling', t0)
         if not full:
             return plans, None, None
         packed = np.packbits(np.concatenate(full), axis=1, bitorder='little')
@@ -287,23 +261,17 @@ def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, t
         for k0 in range(0, K, per_chunk):
             k = min(per_chunk, K - k0)
             rows = k * N_bg
-            end = timer.device('compose') if timer else None
-            check(N.lib.dtb_shap_compose(ptr(x_cat), ptr(x_cont), ptr(bg.cat), ptr(bg.cont), ptr(masks_dev[k0:]),
-                                         bg.words, ptr(index_dev[k0:]), ptr(bg.cat_bit), ptr(bg.cont_bit), k, N_bg,
-                                         F, C, ptr(out_cat), ptr(out_cont), stream_ptr()), 'shap_compose')
-            discrete.rewrite_derived(bg.dt_model.preprocessor, out_cat[:rows] if F else None,
-                                     out_cont[:rows] if C else None)
-            if timer:
-                end.record()
-                end = timer.device('forward')
-            forward_rows(model, out_cat, out_cont, pred[:rows], batch_size)
-            if timer:
-                end.record()
-                end = timer.device('means')
-            check(N.lib.dtb_shap_means(ptr(pred), k, N_bg, bg.cols, bg.kind, ptr(values[k0:]), stream_ptr()),
-                  'shap_means')
-            if timer:
-                end.record()
+            with timer.device('compose'):
+                check(N.lib.dtb_shap_compose(ptr(x_cat), ptr(x_cont), ptr(bg.cat), ptr(bg.cont), ptr(masks_dev[k0:]),
+                                             bg.words, ptr(index_dev[k0:]), ptr(bg.cat_bit), ptr(bg.cont_bit), k,
+                                             N_bg, F, C, ptr(out_cat), ptr(out_cont), stream_ptr()), 'shap_compose')
+                discrete.rewrite_derived(bg.dt_model.preprocessor, out_cat[:rows] if F else None,
+                                         out_cont[:rows] if C else None)
+            with timer.device('forward'):
+                forward_rows(model, out_cat, out_cont, pred[:rows], batch_size)
+            with timer.device('means'):
+                check(N.lib.dtb_shap_means(ptr(pred), k, N_bg, bg.cols, bg.kind, ptr(values[k0:]), stream_ptr()),
+                      'shap_means')
         host = torch.empty(K, dtype=torch.float64, pin_memory=True)
         host.copy_(values, non_blocking=True)
         event = torch.cuda.Event()
@@ -328,8 +296,7 @@ def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, t
                 phi[i, vary[0]] = total
             if trace is not None:
                 trace[i] = Row(vary, masks, weights, y, fx[i])
-        if timer:
-            timer.host['solve'] += time.perf_counter() - t0
+        timer.host('solve', t0)
 
     pending = None
     for g0 in range(0, len(mine), _GROUP_ROWS):
@@ -340,15 +307,8 @@ def shap_values(bg, X, nsamples='auto', seed=0, batch_size=65536, stages=None, t
     if pending is not None:
         finish(pending)
 
-    if world > 1:
-        gathered = [None] * world
-        torch.distributed.all_gather_object(gathered, phi[mine])
-        for r in range(world):
-            phi[r::world] = gathered[r]
-    if stages is not None:
-        torch.cuda.synchronize()
-        stages.update(timer.result())
-    return phi
+    timer.finish()
+    return gather_strided(phi[mine], n_rows)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -366,11 +326,6 @@ def check_gradient_options(dt_model):
         if cfg is not None and getattr(cfg, option, False):
             raise NotImplementedError(f'{option}=True: expected gradients cannot attribute the jumps of its derived '
                                       f'columns')
-
-
-def check_positive_int(value, name):
-    if isinstance(value, bool) or not isinstance(value, numbers.Integral) or value < 1:
-        raise ValueError(f'{name} must be a positive integer, got {value!r}')
 
 
 def gradient_draws(seed, i, nsamples, bg_rows, rng=None):
@@ -428,12 +383,11 @@ def gradient_values(bg, X, nsamples=200, seed=0, batch_size=65536, stages=None):
     phi = np.zeros((n_rows, n_cols, K), np.float64)
     if n_rows == 0:
         return phi
-    timer = _Stages() if stages is not None else None
+    timer = Stages(stages)
     model.flush_optimizer_state()
     t0 = time.perf_counter()
     x_cat, x_cont = bg.encode(X)
-    if timer:
-        timer.host['encode'] += time.perf_counter() - t0
+    timer.host('encode', t0)
     F = x_cat.shape[1] if x_cat is not None else 0
     C = x_cont.shape[1] if x_cont is not None else 0
     emb = _Embeddings(model) if F else None
@@ -441,15 +395,9 @@ def gradient_values(bg, X, nsamples=200, seed=0, batch_size=65536, stages=None):
     bits = np.concatenate([bg.cat_bit.cpu().numpy(), bg.cont_bit.cpu().numpy()])     # frame column of each encoded one
     cols = F + C
 
-    rank, world = (torch.distributed.get_rank(), dp.world_size()) if dp.is_distributed() else (0, 1)
-    mine = list(range(rank, n_rows, world))
+    mine = rank_share(n_rows)
     group_rows = max(1, batch_size // nsamples)
     rng = np.random.RandomState()
-
-    def event(name, end=None):
-        if end is not None:
-            end.record()
-        return timer.device(name) if timer and name else None
 
     def tables():
         return (ptr(x_cat), ptr(x_cont), ptr(bg.cat), ptr(bg.cont), ptr(emb.table) if F else None,
@@ -459,8 +407,7 @@ def gradient_values(bg, X, nsamples=200, seed=0, batch_size=65536, stages=None):
         group = mine[g0:g0 + group_rows]
         t0 = time.perf_counter()
         draws = [gradient_draws(seed, i, nsamples, N_bg, rng) for i in group]
-        if timer:
-            timer.host['draws'] += time.perf_counter() - t0
+        timer.host('draws', t0)
         x_index = torch.as_tensor(np.repeat(np.array(group, np.int32), nsamples)).to(dev)
         bg_index = torch.as_tensor(np.concatenate([d[0] for d in draws])).to(dev)
         alpha = torch.as_tensor(np.concatenate([d[1] for d in draws])).to(dev)
@@ -468,13 +415,13 @@ def gradient_values(bg, X, nsamples=200, seed=0, batch_size=65536, stages=None):
         values = torch.empty(K, P, cols, dtype=torch.float64, device=dev)
         for p0 in range(0, P, batch_size):
             m = min(batch_size, P - p0)
-            end = event('compose')
-            out_emb = torch.empty((F, m, emb.dim) if not emb.ragged else (m, emb.width), dtype=torch.float32,
-                                  device=dev) if F else None
-            out_cont = torch.empty(m, C, dtype=torch.float32, device=dev) if C else None
-            check(N.lib.dtb_gradshap_compose(*tables(), ptr(x_index[p0:]), ptr(bg_index[p0:]), ptr(alpha[p0:]), m, F,
-                                             C, 0 if F and emb.ragged else 1, ptr(out_emb), ptr(out_cont),
-                                             stream_ptr()), 'gradshap_compose')
+            with timer.device('compose'):
+                out_emb = torch.empty((F, m, emb.dim) if not emb.ragged else (m, emb.width), dtype=torch.float32,
+                                      device=dev) if F else None
+                out_cont = torch.empty(m, C, dtype=torch.float32, device=dev) if C else None
+                check(N.lib.dtb_gradshap_compose(*tables(), ptr(x_index[p0:]), ptr(bg_index[p0:]), ptr(alpha[p0:]),
+                                                 m, F, C, 0 if F and emb.ragged else 1, ptr(out_emb), ptr(out_cont),
+                                                 stream_ptr()), 'gradshap_compose')
             inputs = []
             if F:       # the tensor-backed field block reads [F, m, D] in place; its gradient comes back as (m, F, D)
                 out_emb = (out_emb if emb.ragged else out_emb.permute(1, 0, 2)).detach().requires_grad_(True)
@@ -482,42 +429,32 @@ def gradient_values(bg, X, nsamples=200, seed=0, batch_size=65536, stages=None):
             if C:
                 out_cont = out_cont.requires_grad_(True)
                 inputs.append(out_cont)
-            end = event('forward', end)
-            z = model.input_forward(out_emb, out_cont)
-            end = event(None, end)
+            with timer.device('forward'):
+                z = model.input_forward(out_emb, out_cont)
             dz = torch.empty(m, K, dtype=torch.float32, device=dev)
             for k in range(K):
-                end = event('backward')
-                check(N.lib.dtb_gradshap_output_grad(ptr(z.detach()), m, K, k, kind, ptr(dz), stream_ptr()),
+                with timer.device('backward'):
+                    check(N.lib.dtb_gradshap_output_grad(ptr(z.detach()), m, K, k, kind, ptr(dz), stream_ptr()),
                           'gradshap_output_grad')
-                grads = torch.autograd.grad(z, inputs, grad_outputs=dz, retain_graph=k < K - 1, allow_unused=True)
-                grads = [torch.zeros_like(t) if g is None else g.contiguous() for t, g in zip(inputs, grads)]
+                    grads = torch.autograd.grad(z, inputs, grad_outputs=dz, retain_graph=k < K - 1,
+                                                allow_unused=True)
+                    grads = [torch.zeros_like(t) if g is None else g.contiguous() for t, g in zip(inputs, grads)]
                 g_emb = grads[0] if F else None
                 g_cont = grads[-1] if C else None
-                end = event('reduce', end)
-                check(N.lib.dtb_gradshap_reduce(*tables(), ptr(x_index[p0:]), ptr(bg_index[p0:]), m, F, C,
-                                                ptr(g_emb), ptr(g_cont), ptr(values[k, p0:]), stream_ptr()),
-                      'gradshap_reduce')
-                event(None, end)
+                with timer.device('reduce'):
+                    check(N.lib.dtb_gradshap_reduce(*tables(), ptr(x_index[p0:]), ptr(bg_index[p0:]), m, F, C,
+                                                    ptr(g_emb), ptr(g_cont), ptr(values[k, p0:]), stream_ptr()),
+                          'gradshap_reduce')
             del z, inputs
-        end = event('means')
-        means = torch.empty(K, len(group), cols, dtype=torch.float64, device=dev)
-        for k in range(K):
-            check(N.lib.dtb_gradshap_means(ptr(values[k]), len(group), nsamples, cols, ptr(means[k]), stream_ptr()),
-                  'gradshap_means')
-        event(None, end)
+        with timer.device('means'):
+            means = torch.empty(K, len(group), cols, dtype=torch.float64, device=dev)
+            for k in range(K):
+                check(N.lib.dtb_gradshap_means(ptr(values[k]), len(group), nsamples, cols, ptr(means[k]),
+                                               stream_ptr()), 'gradshap_means')
         host = means.cpu().numpy()
         rows = np.array(group)
         for e in range(cols):
             if bits[e] >= 0:
                 phi[rows, bits[e], :] += host[:, :, e].T
-
-    if world > 1:
-        gathered = [None] * world
-        torch.distributed.all_gather_object(gathered, phi[mine])
-        for r in range(world):
-            phi[r::world] = gathered[r]
-    if stages is not None:
-        torch.cuda.synchronize()
-        stages.update(timer.result())
-    return phi
+    timer.finish()
+    return gather_strided(phi[mine], n_rows)

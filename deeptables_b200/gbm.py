@@ -25,6 +25,7 @@ import torch
 
 from . import _native as N, consts, dp
 from ._native import check, ptr, stream_ptr
+from .analysis import Stages, is_int
 
 LEAF_PREFIX = 'lgbm_leaf_'       # hypernets' column naming, as recalled
 
@@ -39,10 +40,6 @@ _IGNORED = ('n_jobs', 'verbose', 'verbosity')
 _NEUTRAL = {'boosting_type': 'gbdt', 'boosting': 'gbdt', 'subsample': 1.0, 'bagging_fraction': 1.0,
             'subsample_freq': 0, 'bagging_freq': 0, 'colsample_bytree': 1.0, 'feature_fraction': 1.0}
 MAX_LEAVES = N.GBDT_STAGE_NODES + 1
-
-
-def _is_int(v):
-    return isinstance(v, numbers.Integral) and not isinstance(v, bool)
 
 
 def _is_real(v):
@@ -71,13 +68,13 @@ def resolve_params(gbm_params, task, num_classes=None):
         out[name] = value
     ints = {'n_estimators': 1, 'num_leaves': 2, 'min_child_samples': 0, 'subsample_for_bin': 1}
     for name, lo in ints.items():
-        if not _is_int(out[name]) or out[name] < lo:
+        if not is_int(out[name]) or out[name] < lo:
             raise ValueError(f'gbm_params {name!r} must be an integer >= {lo}, got {out[name]!r}')
     if out['num_leaves'] > MAX_LEAVES:
         raise ValueError(f'gbm_params num_leaves must be at most {MAX_LEAVES}, got {out["num_leaves"]}')
-    if not _is_int(out['max_depth']):
+    if not is_int(out['max_depth']):
         raise ValueError(f'gbm_params max_depth must be an integer (<= 0: no limit), got {out["max_depth"]!r}')
-    if not _is_int(out['max_bin']) or out['max_bin'] < 2:
+    if not is_int(out['max_bin']) or out['max_bin'] < 2:
         raise ValueError(f'gbm_params max_bin must be an integer >= 2, got {out["max_bin"]!r}')
     if out['max_bin'] > 255:
         raise NotImplementedError(f'gbm_params max_bin = {out["max_bin"]}: bins are uint8, at most 255 are built')
@@ -89,7 +86,7 @@ def resolve_params(gbm_params, task, num_classes=None):
         out[name] = float(out[name])
     out['learning_rate'] = float(out['learning_rate'])
     rs = out['random_state']
-    if rs is not None and (not _is_int(rs) or not 0 <= rs < 2 ** 32):
+    if rs is not None and (not is_int(rs) or not 0 <= rs < 2 ** 32):
         raise ValueError(f'gbm_params random_state must be None or an integer in [0, 2**32), got {rs!r}')
     if task == consts.TASK_MULTICLASS and 'n_estimators' not in given:
         out['n_estimators'] = int(100 / num_classes) + 1      # hypernets' encoder, as recalled
@@ -214,34 +211,25 @@ class Booster:
         self.edges_d = torch.as_tensor(flat).to(device)
         self.edge_off_d = torch.as_tensor(off).to(device)
         self.n_bins_d = torch.as_tensor(self.n_bins).to(device)
-        self.timer = None       # name -> [(start, end) CUDA events], set by tools/bench_gbm.py
-
-    def _t(self, name):
-        if self.timer is None:
-            return None
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        self.timer.setdefault(name, []).append((s, e))
-        return e
 
     def bin(self, cat, cont, rows):
         bins = torch.empty(rows, self.nf, dtype=torch.uint8, device=self.device)
-        end = self._t('bin')
         check(N.lib.dtb_gbdt_bin(ptr(cat), cat.shape[1] if cat is not None else 0, ptr(cont),
                                  cont.shape[1] if cont is not None else 0, ptr(self.feat_col_d), ptr(self.edges_d),
                                  ptr(self.edge_off_d), rows, self.nf, ptr(bins), stream_ptr()), 'gbdt_bin')
-        if end is not None:
-            end.record()
         return bins
 
-    def fit(self, cat, cont, label, leaf_log=None):
+    def fit(self, cat, cont, label, leaf_log=None, stages=None):
         """Trees fitted to ``label`` (numpy: 0/1, the target, or class codes).  ``leaf_log``: an int32 [rows, trees]
-        device tensor, or None; it receives each training row's leaf from the partition, tree by tree."""
+        device tensor, or None; it receives each training row's leaf from the partition, tree by tree.  ``stages``: a
+        dict that receives the seconds spent in bin, grad, hist, split, partition and update (CUDA events)."""
         p, K, dev = self.p, self.K, self.device
         rows = len(label)
         if rows >= 2 ** 31:
             raise ValueError('the booster takes fewer than 2**31 rows')
-        bins = self.bin(cat, cont, rows)
+        timer = Stages(stages)
+        with timer.device('bin'):
+            bins = self.bin(cat, cont, rows)
         y = torch.as_tensor(np.asarray(label, np.float32)).to(dev)
         scores = torch.empty(rows, K, dtype=torch.float64, device=dev)
         scores[:] = torch.as_tensor(init_scores(np.asarray(label), self.task, K), device=dev)
@@ -266,38 +254,32 @@ class Booster:
         def split(leaves, sp):
             pair_host[:len(leaves)] = torch.tensor(leaves, dtype=torch.int32)
             pair[:len(leaves)].copy_(pair_host[:len(leaves)], non_blocking=True)
-            end = self._t('split')
-            check(N.lib.dtb_gbdt_split(ptr(hg), ptr(hh), ptr(hn), ptr(pair), len(leaves), ptr(self.n_bins_d),
-                                       self.nf, self.nb, ctypes.byref(sp), ptr(recs), stream_ptr()), 'gbdt_split')
-            if end is not None:
-                end.record()
+            with timer.device('split'):
+                check(N.lib.dtb_gbdt_split(ptr(hg), ptr(hh), ptr(hn), ptr(pair), len(leaves), ptr(self.n_bins_d),
+                                           self.nf, self.nb, ctypes.byref(sp), ptr(recs), stream_ptr()), 'gbdt_split')
             recs_host.copy_(recs)           # synchronises: the host picks the next leaf from these records
             raw = recs_host.numpy().tobytes()
             size = ctypes.sizeof(N.GbdtSplitRec)
             return [N.GbdtSplitRec.from_buffer_copy(raw[i * size:(i + 1) * size]) for i in range(len(leaves))]
 
         def hist(slot, begin, count):
-            end = self._t('hist')
-            check(N.lib.dtb_gbdt_hist(ptr(bins), ptr(index), begin, count, ptr(gq), ptr(hq), self.nf, self.nb,
-                                      ptr(hg[slot]), ptr(hh[slot]), ptr(hn[slot]), stream_ptr()), 'gbdt_hist')
-            if end is not None:
-                end.record()
+            with timer.device('hist'):
+                check(N.lib.dtb_gbdt_hist(ptr(bins), ptr(index), begin, count, ptr(gq), ptr(hq), self.nf, self.nb,
+                                          ptr(hg[slot]), ptr(hh[slot]), ptr(hn[slot]), stream_ptr()), 'gbdt_hist')
 
         for it in range(p['n_estimators']):
             maxgh.zero_()
-            end = self._t('grad')
-            for k in range(K):     # every class's gradient from the scores before this iteration's trees (LightGBM)
-                check(N.lib.dtb_gbdt_grad(ptr(scores), ptr(y), rows, K, k, self.objective, ptr(g[k]), ptr(h[k]),
-                                          ptr(maxgh[k]), stream_ptr()), 'gbdt_grad')
-            if end is not None:
-                end.record()
+            with timer.device('grad'):
+                for k in range(K):   # every class's gradient from the scores before this iteration's trees (LightGBM)
+                    check(N.lib.dtb_gbdt_grad(ptr(scores), ptr(y), rows, K, k, self.objective, ptr(g[k]), ptr(h[k]),
+                                              ptr(maxgh[k]), stream_ptr()), 'gbdt_grad')
             m = maxgh.cpu().numpy()
             grown = []
             for k in range(K):      # each tree updates its class's scores at once; the gradients were taken above
                 tree = self._grow(k, rows, m[k], g[k], h[k], gq, hq, arange, index, scratch, hist, split, hg, hh, hn,
-                                  bins)
+                                  bins, timer)
                 if tree is not None:
-                    self._update(tree, index, scores, k, leaf_log, len(trees) + k)
+                    self._update(tree, index, scores, k, leaf_log, len(trees) + k, timer)
                 grown.append(tree)
             if all(t is None for t in grown):
                 break           # no root meets the split requirements: boosting stops, as in LightGBM
@@ -308,28 +290,25 @@ class Booster:
                     if leaf_log is not None:
                         leaf_log[:, len(trees)] = 0
                 trees.append(tree)
+        timer.finish()
         return _trees_from_lists(trees)
 
-    def _update(self, tree, index, scores, k, leaf_log, column):
+    def _update(self, tree, index, scores, k, leaf_log, column, timer):
         dev = self.device
         values = torch.as_tensor(np.asarray(tree['values'], np.float32)).to(dev)
         seg_b = torch.as_tensor(np.asarray(tree['seg_begin'], np.int64)).to(dev)
         seg_c = torch.as_tensor(np.asarray(tree['seg_count'], np.int64)).to(dev)
         col = leaf_log[:, column] if leaf_log is not None else None
-        end = self._t('update')
-        check(N.lib.dtb_gbdt_update(ptr(index), ptr(seg_b), ptr(seg_c), len(tree['values']), int(max(tree['seg_count'])),
-                                    ptr(values), ptr(scores), self.K, k, ptr(col),
-                                    leaf_log.shape[1] if leaf_log is not None else 0, stream_ptr()), 'gbdt_update')
-        if end is not None:
-            end.record()
+        with timer.device('update'):
+            check(N.lib.dtb_gbdt_update(ptr(index), ptr(seg_b), ptr(seg_c), len(tree['values']),
+                                        int(max(tree['seg_count'])), ptr(values), ptr(scores), self.K, k, ptr(col),
+                                        leaf_log.shape[1] if leaf_log is not None else 0, stream_ptr()), 'gbdt_update')
 
-    def _grow(self, k, rows, m, g, h, gq, hq, arange, index, scratch, hist, split, hg, hh, hn, bins):
+    def _grow(self, k, rows, m, g, h, gq, hq, arange, index, scratch, hist, split, hg, hh, hn, bins, timer):
         p = self.p
         sg, sh = fixed_shift(m[0], rows), fixed_shift(m[1], rows)
-        end = self._t('grad')
-        check(N.lib.dtb_gbdt_fixed(ptr(g), ptr(h), rows, sg, sh, ptr(gq), ptr(hq), stream_ptr()), 'gbdt_fixed')
-        if end is not None:
-            end.record()
+        with timer.device('grad'):
+            check(N.lib.dtb_gbdt_fixed(ptr(g), ptr(h), rows, sg, sh, ptr(gq), ptr(hq), stream_ptr()), 'gbdt_fixed')
         sp = N.GbdtSplitParams(p['reg_lambda'], p['reg_alpha'], p['min_split_gain'], p['min_child_weight'],
                                2.0 ** -sg, 2.0 ** -sh, p['min_child_samples'])
         index.copy_(arange)
@@ -351,11 +330,9 @@ class Booster:
                 break
             lf, new = leaves[best], len(leaves)
             r = lf['rec']
-            end = self._t('partition')
-            check(N.lib.dtb_gbdt_partition(ptr(bins), self.nf, ptr(index), lf['begin'], lf['count'], r.feature, r.bin,
-                                           r.left_count, ptr(scratch), stream_ptr()), 'gbdt_partition')
-            if end is not None:
-                end.record()
+            with timer.device('partition'):
+                check(N.lib.dtb_gbdt_partition(ptr(bins), self.nf, ptr(index), lf['begin'], lf['count'], r.feature,
+                                               r.bin, r.left_count, ptr(scratch), stream_ptr()), 'gbdt_partition')
             node = len(feature)
             feature.append(r.feature)
             bin_.append(r.bin)
@@ -373,11 +350,10 @@ class Booster:
             small_is_left = lc <= rc
             small = lf if small_is_left else right_leaf
             hist(new, small['begin'], small['count'])
-            end = self._t('hist')
-            check(N.lib.dtb_gbdt_hist_sub(ptr(hg[best]), ptr(hh[best]), ptr(hn[best]), ptr(hg[new]), ptr(hh[new]),
-                                          ptr(hn[new]), hg.shape[1], int(small_is_left), stream_ptr()), 'gbdt_hist_sub')
-            if end is not None:
-                end.record()
+            with timer.device('hist'):
+                check(N.lib.dtb_gbdt_hist_sub(ptr(hg[best]), ptr(hh[best]), ptr(hn[best]), ptr(hg[new]), ptr(hh[new]),
+                                              ptr(hn[new]), hg.shape[1], int(small_is_left), stream_ptr()),
+                      'gbdt_hist_sub')
             lf['rec'], right_leaf['rec'] = split([best, new], sp)
         values = [leaf_value(lf['rec'].g, lf['rec'].h, sg, sh, p) for lf in leaves]
         return {'feature': feature, 'bin': bin_, 'threshold': thr, 'left': left, 'right': right, 'gain': gain,

@@ -13,13 +13,14 @@ Data parallel: every rank calls this with the same frame; pass ``s`` (0 is the u
 """
 import collections
 import ctypes
-import numbers
 
 import numpy as np
 import torch
 
-from . import _native as N, consts, discrete, dp, engine as E, metrics as M
+from . import _native as N, consts, discrete, engine as E, metrics as M
 from ._native import check, ptr, stream_ptr
+from .analysis import check_positive_int, draw_seed, fitted_model, forward_rows, gather_strided, model_columns, \
+    rank_share
 
 AUC, LOG_LOSS, ACCURACY, F1, F1_MACRO, MSE, RMSE, MAE, R2 = range(1, 10)     # DTB_IMPORTANCE_* (deeptables_b200.h)
 STREAMING, AUC_OVO = 0, -1     # streaming metrics of metrics.py; multiclass one-vs-one AUC (scikit-learn, host)
@@ -70,22 +71,6 @@ def resolve_metric(metric, task, num_classes):
     raise ValueError(f'Unsupported metric: {metric!r}')
 
 
-def draw_seed(random_state):
-    """The 32-bit seed of the permutations: ``random_state`` itself, or (None) one drawn from numpy's global generator,
-    rank 0's under data parallel."""
-    if random_state is None:
-        seed = int(np.random.randint(0, 2 ** 32, dtype=np.uint64))
-        if dp.is_distributed():
-            box = [seed]
-            torch.distributed.broadcast_object_list(box, src=0)
-            seed = int(box[0])
-        return seed
-    if isinstance(random_state, bool) or not isinstance(random_state, numbers.Integral) or \
-            not 0 <= random_state < 2 ** 32:
-        raise ValueError(f'random_state must be None or an integer in [0, 2**32), got {random_state!r}')
-    return int(random_state)
-
-
 def _sorted_keys(rows, seed, iteration, column, device):
     """The keys of pass (iteration, column) in ascending order: their low halves are its permutation."""
     keys = torch.empty(rows, dtype=torch.int64, device=device)
@@ -96,20 +81,6 @@ def _sorted_keys(rows, seed, iteration, column, device):
 def permutation(rows, seed, iteration, column, device):
     """The permutation of pass (iteration, column): int64 [rows] on ``device``; row b of the pass reads row perm[b]."""
     return _sorted_keys(rows, seed, iteration, column, device) & 0xFFFFFFFF
-
-
-def forward_rows(model, cat, cont, pred, batch_size):
-    """The inference forward of ``model`` over the first ``len(pred)`` rows of the device inputs ``cat`` / ``cont``
-    (either may be None), ``batch_size`` rows per call, its outputs written into ``pred`` [rows, cols] float32.  The
-    caller brings the embedding rows up to date first (``model.flush_optimizer_state()``)."""
-    with torch.no_grad():
-        for lo in range(0, pred.shape[0], batch_size):
-            hi = min(lo + batch_size, pred.shape[0])
-            bc = cat[lo:hi] if cat is not None else None
-            bx = cont[lo:hi] if cont is not None else None
-            z = model._forward(bc, bx, training=False)
-            p, _ = E.loss_forward_backward(z, torch.zeros_like(z), model.task, None, False, None)
-            pred[lo:hi].copy_(p)
 
 
 def _class_ranks(labels):
@@ -159,13 +130,9 @@ def score_decreases(dt_model, X, y, metric, n_iter=5, mode='min', random_state=N
     rank, seed).  Columns the model does not read decrease by exactly 0.0 and cost no pass."""
     if mode not in ('min', 'max'):
         raise ValueError(f'Unsupported mode:{mode}')
-    if isinstance(n_iter, bool) or not isinstance(n_iter, numbers.Integral) or n_iter < 1:
-        raise ValueError(f'n_iter must be a positive integer, got {n_iter!r}')
-    if isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral) or batch_size < 1:
-        raise ValueError(f'batch_size must be a positive integer, got {batch_size!r}')
-    model = dt_model.get_model()
-    if model is None or model.model is None:
-        raise ValueError('the DeepTable has no fitted model')
+    check_positive_int(n_iter, 'n_iter')
+    check_positive_int(batch_size, 'batch_size')
+    model = fitted_model(dt_model)
     scorer = resolve_metric(metric, model.task, model.num_classes)
     if scorer.kind == AUC and model.task == consts.TASK_MULTICLASS:
         scorer = scorer._replace(kind=AUC_OVO)
@@ -180,8 +147,7 @@ def score_decreases(dt_model, X, y, metric, n_iter=5, mode='min', random_state=N
     targets = _Targets(dt_model, model, y, scorer, device)
 
     cat, cont = model._to_device_inputs(dt_model.preprocessor.transform_X(X))
-    cat_names = [c.name for c in model.categorical_columns]
-    cont_names = [name for c in model.continuous_columns for name in c.column_names]
+    cat_names, cont_names = model_columns(model)
     read = []                                   # (position in X, working array key, column in that array)
     for j, c in enumerate(columns):
         if str(c) in cat_names:
@@ -227,9 +193,9 @@ def score_decreases(dt_model, X, y, metric, n_iter=5, mode='min', random_state=N
                                             targets.aux, ptr(scratch), out, stream_ptr()), 'importance_sums')
 
     model.flush_optimizer_state()               # every embedding row current: the forward needs no per-batch catch-up
-    rank, world = (torch.distributed.get_rank(), dp.world_size()) if dp.is_distributed() else (0, 1)
+    mine = rank_share(n_slots)
     passes = 0
-    for slot in range(rank, n_slots, world):
+    for slot in mine:
         if slot == 0:
             forward()
         else:
@@ -246,18 +212,14 @@ def score_decreases(dt_model, X, y, metric, n_iter=5, mode='min', random_state=N
             passes += 1
         score(slot)
 
-    values = scores.cpu().numpy()
-    for slot, v in host_scores.items():
-        values[slot] = v
-    raw_states = states.cpu().numpy().view(np.uint64) if states is not None else None
-    if world > 1:
-        gathered = [None] * world
-        torch.distributed.all_gather_object(gathered, (values, raw_states))
-        values = np.array([gathered[s % world][0][s] for s in range(n_slots)], np.float64)
-        if raw_states is not None:
-            raw_states = np.stack([gathered[s % world][1][s] for s in range(n_slots)])
-    if raw_states is not None:
+    if states is not None:
+        raw_states = gather_strided(states.cpu().numpy().view(np.uint64)[mine], n_slots)
         values = np.array([float(state.plan.finish(raw_states[s])[scorer.spec.key]) for s in range(n_slots)])
+    else:
+        values = scores.cpu().numpy()
+        for slot, v in host_scores.items():
+            values[slot] = v
+        values = gather_strided(values[mine], n_slots)
     signed = -values if mode == 'min' else values
     decreases = np.zeros((n_iter, len(columns)), np.float64)
     for i in range(n_slots - 1):

@@ -25,19 +25,13 @@ import numpy as np
 import pandas as pd
 import torch
 
-from .. import _native as N, discrete, dp
+from .. import _native as N, discrete
 from .._native import check, ptr, stream_ptr
-from ..importance import forward_rows
+from ..analysis import Stages, check_positive_int, fitted_model, forward_rows, gather_strided, is_int, model_columns, \
+    rank_share
 
 _BLOCK_ROWS = 1024        # X rows per float64 block sum; chunks of rows start on multiples of it
 _KINDS = ('average', 'individual', 'both')
-
-
-def _fitted_model(dt_model):
-    model = dt_model.get_model() if dt_model is not None else None
-    if model is None or isinstance(model, list) or getattr(model, 'model', None) is None:
-        raise ValueError('dt_model: the DeepTable has no fitted model')
-    return model
 
 
 def _as_frame(X, feature_names):
@@ -64,17 +58,13 @@ def _check_columns(dt_model, X):
         raise ValueError(f'X lacks the columns {missing} the model was fitted on')
 
 
-def _is_int(v):
-    return isinstance(v, numbers.Integral) and not isinstance(v, (bool, np.bool_))
-
-
 def feature_indices(columns, features):
     """Positions in ``columns`` of ``features`` (an int, a str, a bool mask, or a list of ints or of strs) and the key
     of each in ``custom_values`` (the element as given; the position for a mask)."""
     names = [str(c) for c in columns]
 
     def one(f):
-        if _is_int(f):
+        if is_int(f):
             if not 0 <= f < len(names):
                 raise ValueError(f'features: index {f} is not in [0, {len(names) - 1}]')
             return int(f)
@@ -84,7 +74,7 @@ def feature_indices(columns, features):
             return names.index(f)
         raise ValueError(f'features: {f!r} is not an int, a str or a bool mask')
 
-    if _is_int(features) or isinstance(features, str):
+    if is_int(features) or isinstance(features, str):
         return [one(features)], [features]
     flist = list(features) if isinstance(features, Iterable) else [features]
     if not flist:
@@ -96,7 +86,7 @@ def feature_indices(columns, features):
         if not idx:
             raise ValueError('features: the bool mask selects no feature')
         return idx, idx
-    if not (all(_is_int(f) for f in flist) or all(isinstance(f, str) for f in flist)):
+    if not (all(is_int(f) for f in flist) or all(isinstance(f, str) for f in flist)):
         raise ValueError('features: a list of features holds ints or strs, not both')
     return [one(f) for f in flist], flist
 
@@ -128,7 +118,7 @@ def _check_percentiles(percentiles):
 
 
 def _check_grid_resolution(grid_resolution):
-    if not _is_int(grid_resolution) or grid_resolution <= 1:
+    if not is_int(grid_resolution) or grid_resolution <= 1:
         raise ValueError(f'grid_resolution must be an integer strictly greater than 1, got {grid_resolution!r}')
 
 
@@ -218,7 +208,7 @@ def _partial_dependence(dt_model, X, features, *, sample_weight, categorical_fea
     clock) and in compose, forward and reduce (CUDA events)."""
     from sklearn.utils import Bunch
     from .. import consts
-    model = _fitted_model(dt_model)
+    model = fitted_model(dt_model)
     regression = model.task == consts.TASK_REGRESSION
     if method == 'recursion':
         raise ValueError("method='recursion' needs a tree-based estimator; use method='brute' or 'auto'")
@@ -232,8 +222,7 @@ def _partial_dependence(dt_model, X, features, *, sample_weight, categorical_fea
         raise ValueError("response_method is ignored for regression and must be 'auto'")
     if kind not in _KINDS:
         raise ValueError(f'kind must be one of {_KINDS}, got {kind!r}')
-    if isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral) or batch_size < 1:
-        raise ValueError(f'batch_size must be a positive integer, got {batch_size!r}')
+    check_positive_int(batch_size, 'batch_size')
     if custom_values is not None and not isinstance(custom_values, dict):
         raise ValueError('custom_values must be a dict or None')
     _check_percentiles(percentiles)
@@ -263,28 +252,6 @@ def _partial_dependence(dt_model, X, features, *, sample_weight, categorical_fea
     return out
 
 
-class _Timer:
-    """CUDA events around the device stages."""
-
-    def __init__(self, stages):
-        self.stages, self.events = stages, []
-
-    def __call__(self, name):
-        if self.stages is None:
-            return None
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        self.events.append((name, start, end))
-        return end
-
-    def finish(self):
-        if self.stages is None:
-            return
-        torch.cuda.synchronize()
-        for name, start, end in self.events:
-            self.stages[name] = self.stages.get(name, 0.0) + start.elapsed_time(end) / 1e3
-
-
 def block_sums(pred, weight, groups, rows_per_group, out):
     """``dtb_pdp_block_sums`` of ``pred`` [groups*rows_per_group, cols] into the float64 device tensor ``out``
     (``groups * blocks * cols`` elements from its start)."""
@@ -305,7 +272,7 @@ def _device_pd(dt_model, model, X, idx, grid, weight, individual, batch_size, st
     dev, pre = model.device, dt_model.preprocessor
     n, G, cols = len(X), len(grid), model._output_dim()
     nb = (n + _BLOCK_ROWS - 1) // _BLOCK_ROWS
-    timer = _Timer(stages)
+    timer = Stages(stages)
     t0 = time.perf_counter()
     model.flush_optimizer_state()       # every embedding row current: the forward needs no per-batch catch-up
     x_cat, x_cont = model._to_device_inputs(pre.transform_X(X))
@@ -318,23 +285,18 @@ def _device_pd(dt_model, model, X, idx, grid, weight, individual, batch_size, st
         w_total = float(add_blocks(w_blocks.cpu().numpy().reshape(1, nb, 1))[0, 0])
 
     names = {str(X.columns[j]) for j in idx}
-    cat_names = [c.name for c in model.categorical_columns]
-    cont_names = [name for c in model.continuous_columns for name in c.column_names]
+    cat_names, cont_names = model_columns(model)
     cat_bit = [0 if c in names else -1 for c in cat_names]
     cont_bit = [0 if c in names else -1 for c in cont_names]
 
     if 0 not in cat_bit + cont_bit:
         # no feature column is read: every grid point's rows are X's own, so every point has X's mean
         pred = torch.empty(n, cols, dtype=torch.float32, device=dev)
-        end = timer('forward')
-        forward_rows(model, x_cat, x_cont, pred, batch_size)
-        if end is not None:
-            end.record()
-            end = timer('reduce')
+        with timer.device('forward'):
+            forward_rows(model, x_cat, x_cont, pred, batch_size)
         sums = torch.empty(nb * cols, dtype=torch.float64, device=dev)
-        block_sums(pred, w_dev, 1, n, sums)
-        if end is not None:
-            end.record()
+        with timer.device('reduce'):
+            block_sums(pred, w_dev, 1, n, sums)
         mean = add_blocks(sums.cpu().numpy().reshape(1, nb, cols))[0] / w_total
         timer.finish()
         avg = np.repeat(mean[:, None], G, axis=1)
@@ -345,13 +307,11 @@ def _device_pd(dt_model, model, X, idx, grid, weight, individual, batch_size, st
     for i, j in enumerate(idx):
         frame.isetitem(j, grid[:, i])
     g_cat, g_cont = model._to_device_inputs(pre.transform_X(frame))
-    if stages is not None:
-        stages['encode'] = stages.get('encode', 0.0) + time.perf_counter() - t0
+    timer.host('encode', t0)
     cat_bit = torch.tensor(cat_bit, dtype=torch.int32, device=dev)
     cont_bit = torch.tensor(cont_bit, dtype=torch.int32, device=dev)
 
-    rank, world = (torch.distributed.get_rank(), dp.world_size()) if dp.is_distributed() else (0, 1)
-    mine = np.arange(rank, G, world)
+    mine = rank_share(G)
     cap = max(batch_size, _BLOCK_ROWS)
     if n <= cap:
         row_step, per = n, max(1, cap // n)            # all rows of X, several grid points per chunk
@@ -364,7 +324,7 @@ def _device_pd(dt_model, model, X, idx, grid, weight, individual, batch_size, st
     out_cont = torch.empty(buf_rows, C, dtype=torch.float32, device=dev) if C else None
     pred = torch.empty(buf_rows, cols, dtype=torch.float32, device=dev)
     masks = torch.ones(per, dtype=torch.int32, device=dev)          # one mask word per grid point: bit 0
-    index = torch.as_tensor(mine.astype(np.int32)).to(dev)
+    index = torch.as_tensor(np.array(mine, np.int32)).to(dev)
     sums = torch.empty(len(mine) * nb * cols, dtype=torch.float64, device=dev)
     ice = np.empty((cols, n, len(mine)), np.float32) if individual else None
 
@@ -373,36 +333,20 @@ def _device_pd(dt_model, model, X, idx, grid, weight, individual, batch_size, st
         for r0 in range(0, n, row_step):
             m = min(row_step, n - r0)
             rows = k * m
-            end = timer('compose')
-            check(N.lib.dtb_shap_compose(ptr(g_cat), ptr(g_cont), ptr(x_cat[r0:] if F else None),
-                                         ptr(x_cont[r0:] if C else None), ptr(masks), 1, ptr(index[i0:]),
-                                         ptr(cat_bit), ptr(cont_bit), k, m, F, C, ptr(out_cat), ptr(out_cont),
-                                         stream_ptr()), 'shap_compose')
-            discrete.rewrite_derived(pre, out_cat[:rows] if F else None, out_cont[:rows] if C else None)
-            if end is not None:
-                end.record()
-                end = timer('forward')
-            forward_rows(model, out_cat, out_cont, pred[:rows], batch_size)
-            if end is not None:
-                end.record()
-                end = timer('reduce')
-            block_sums(pred[:rows], w_dev[r0:] if w_dev is not None else None, k, m,
-                       sums[(i0 * nb + r0 // _BLOCK_ROWS) * cols:])
-            if end is not None:
-                end.record()
+            with timer.device('compose'):
+                check(N.lib.dtb_shap_compose(ptr(g_cat), ptr(g_cont), ptr(x_cat[r0:] if F else None),
+                                             ptr(x_cont[r0:] if C else None), ptr(masks), 1, ptr(index[i0:]),
+                                             ptr(cat_bit), ptr(cont_bit), k, m, F, C, ptr(out_cat), ptr(out_cont),
+                                             stream_ptr()), 'shap_compose')
+                discrete.rewrite_derived(pre, out_cat[:rows] if F else None, out_cont[:rows] if C else None)
+            with timer.device('forward'):
+                forward_rows(model, out_cat, out_cont, pred[:rows], batch_size)
+            with timer.device('reduce'):
+                block_sums(pred[:rows], w_dev[r0:] if w_dev is not None else None, k, m,
+                           sums[(i0 * nb + r0 // _BLOCK_ROWS) * cols:])
             if individual:
                 ice[:, r0:r0 + m, i0:i0 + k] = pred[:rows].view(k, m, cols).permute(2, 1, 0).cpu().numpy()
 
     avg_mine = (add_blocks(sums.cpu().numpy().reshape(len(mine), nb, cols)) / w_total).T       # [cols, mine]
     timer.finish()
-    if world == 1:
-        return avg_mine, ice
-    gathered = [None] * world
-    torch.distributed.all_gather_object(gathered, (avg_mine, ice))
-    avg = np.empty((cols, G), np.float64)
-    full = np.empty((cols, n, G), np.float32) if individual else None
-    for r in range(world):
-        avg[:, r::world] = gathered[r][0]
-        if individual:
-            full[:, :, r::world] = gathered[r][1]
-    return avg, full
+    return gather_strided(avg_mine, G, 1), gather_strided(ice, G, 2) if individual else None

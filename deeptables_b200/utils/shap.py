@@ -7,12 +7,11 @@ regression, the class code on the classification tasks.  Differences from shap: 
 coalitions are sampled, the identity link only, one output only, and the random coalitions are drawn from a generator
 seeded per explained row (``random_state``), not from numpy's global one.
 """
-import numbers
-
 import numpy as np
 import pandas as pd
 
-from .. import explain, importance
+from .. import explain
+from ..analysis import check_positive_int, draw_seed, is_int
 
 
 class KernelExplainer:
@@ -23,22 +22,27 @@ class KernelExplainer:
         self.expected_value = np.float64(expected_value)
 
 
-def _check_explainer_args(random_state, batch_size, num_samples):
-    if random_state is not None:
-        importance.draw_seed(random_state)                  # validates it
-    if isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral) or batch_size < 1:
-        raise ValueError(f'batch_size must be a positive integer, got {batch_size!r}')
-    if num_samples is not None and (isinstance(num_samples, bool) or not isinstance(num_samples, numbers.Integral)
-                                    or num_samples < 1):
-        raise ValueError(f'num_samples must be None or a positive integer, got {num_samples!r}')
-
-
 def _background_rows(X, num_samples):
     """shap.sample's rule: ``num_samples`` rows of X drawn without replacement with random_state 0, or all of X."""
     if num_samples is not None and num_samples < len(X):
         from sklearn.utils import resample
         return resample(X, n_samples=num_samples, random_state=0, replace=False)
     return X
+
+
+def _init_explainer(ex, dt_model, X, num_samples, random_state, batch_size):
+    """What both explainers check and set up: the arguments, the attributes and the background."""
+    if random_state is not None:
+        draw_seed(random_state)                             # validates it
+    check_positive_int(batch_size, 'batch_size')
+    if num_samples is not None and (not is_int(num_samples) or num_samples < 1):
+        raise ValueError(f'num_samples must be None or a positive integer, got {num_samples!r}')
+    ex.dt_model = dt_model
+    ex.num_samples = num_samples
+    ex.feature_names = X.columns.to_list()
+    ex.random_state = random_state
+    ex.batch_size = int(batch_size)
+    ex._background = explain.Background(dt_model, _background_rows(X, num_samples), ex.batch_size)
 
 
 def _as_frame(X, feature_names):
@@ -56,13 +60,7 @@ class DeepTablesExplainer:
         ``random_state``: an int in [0, 2**32) seeding the random coalitions, or None for a seed drawn from numpy's
         global generator at each ``get_shap_values`` call (rank 0's under data parallel).  ``batch_size``: rows per
         forward call."""
-        _check_explainer_args(random_state, batch_size, num_samples)
-        self.dt_model = dt_model
-        self.num_samples = num_samples
-        self.feature_names = X.columns.to_list()
-        self.random_state = random_state
-        self.batch_size = int(batch_size)
-        self._background = explain.Background(dt_model, _background_rows(X, num_samples), self.batch_size)
+        _init_explainer(self, dt_model, X, num_samples, random_state, batch_size)
         self.explainer = KernelExplainer(self._background.expected)
 
     def model_fn(self, data_asarray):
@@ -77,7 +75,7 @@ class DeepTablesExplainer:
         columns) or a positive int, at most 2^M - 2 when M <= 30."""
         explain.check_nsamples(nsamples)
         X_to_explain = _as_frame(X_to_explain, self.feature_names)
-        seed = importance.draw_seed(self.random_state)
+        seed = draw_seed(self.random_state)
         return explain.shap_values(self._background, X_to_explain, nsamples, seed, self.batch_size)
 
 
@@ -103,14 +101,8 @@ class DeepTablesGradientExplainer:
 
         Attributes: ``dt_model``, ``num_samples``, ``feature_names`` and, beyond shap's, ``expected_value``: the float64
         mean of the explained output over the background (a scalar, or one value per output column)."""
-        _check_explainer_args(random_state, batch_size, num_samples)
         explain.check_gradient_options(dt_model)
-        self.dt_model = dt_model
-        self.num_samples = num_samples
-        self.feature_names = X.columns.to_list()
-        self.random_state = random_state
-        self.batch_size = int(batch_size)
-        self._background = explain.Background(dt_model, _background_rows(X, num_samples), self.batch_size)
+        _init_explainer(self, dt_model, X, num_samples, random_state, batch_size)
         bg = self._background
         means = explain.output_means(bg, bg.cat, bg.cont, bg.rows, self.batch_size)
         self.expected_value = np.float64(means[0]) if bg.cols == 1 else means
@@ -121,11 +113,11 @@ class DeepTablesGradientExplainer:
         n_outputs)`` on multiclass and multilabel ones (output column last; shap's own layout for several outputs
         differs between its versions).  ``nsamples``: samples per row, a positive int.  Each row sums to about the
         output at that row minus ``expected_value``; the error shrinks as ``nsamples`` grows."""
-        explain.check_positive_int(nsamples, 'nsamples')
+        check_positive_int(nsamples, 'nsamples')
         X_to_explain = _as_frame(X_to_explain, self.feature_names)
         if X_to_explain.columns.to_list() != self._background.columns:
             raise ValueError(f'X_to_explain has columns {X_to_explain.columns.to_list()}, the explainer '
                              f'{self._background.columns}')
-        seed = importance.draw_seed(self.random_state)
+        seed = draw_seed(self.random_state)
         phi = explain.gradient_values(self._background, X_to_explain, nsamples, seed, self.batch_size)
         return phi[:, :, 0] if self._background.cols == 1 else phi

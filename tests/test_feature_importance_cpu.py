@@ -67,15 +67,25 @@ def test_metric_validation():
 
 
 def test_seed_validation():
-    from deeptables_b200 import importance as I
-    assert I.draw_seed(0) == 0 and I.draw_seed(2 ** 32 - 1) == 2 ** 32 - 1
+    from deeptables_b200.analysis import draw_seed
+    assert draw_seed(0) == 0 and draw_seed(2 ** 32 - 1) == 2 ** 32 - 1
     np.random.seed(3)
-    a = I.draw_seed(None)
+    a = draw_seed(None)
     np.random.seed(3)
-    assert I.draw_seed(None) == a
+    assert draw_seed(None) == a
     for bad in (-1, 2 ** 32, 1.5, True, 'x'):
         with pytest.raises(ValueError):
-            I.draw_seed(bad)
+            draw_seed(bad)
+
+
+def test_a_model_set_is_not_a_fitted_model():
+    from deeptables_b200 import importance
+
+    class ModelSet:
+        def get_model(self):
+            return [object()]
+    with pytest.raises(ValueError, match='no fitted model'):
+        importance.score_decreases(ModelSet(), None, None, 'auc')
 
 
 def test_restated_keys_give_a_permutation_that_depends_on_every_input():

@@ -266,10 +266,10 @@ def _fitted(task, nets='DeepFM', **kw):
 
 def _outputs(dt, frame):
     """The explained output of each row on the host: [rows, outputs] float64."""
-    from deeptables_b200 import explain
+    from deeptables_b200 import analysis, explain
     bg = explain.Background(dt, frame, 65536)
     pred = torch.empty(len(frame), bg.cols, dtype=torch.float32, device='cuda')
-    explain.forward_rows(bg.model, bg.cat, bg.cont, pred, 65536)
+    analysis.forward_rows(bg.model, bg.cat, bg.cont, pred, 65536)
     return pred.cpu().numpy().astype(np.float64)
 
 

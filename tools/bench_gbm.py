@@ -5,7 +5,7 @@
 
 Prints, with the card's name and power limit:
 - the booster fit on the encoded device inputs, split into bin / grad / hist / split / partition / update (CUDA events
-  around each launch) and the host's share;
+  around each launch, in a second fit) and the host's share;
 - the histogram kernel on the root (all rows) over 20 launches: bytes/s of the algorithmic bytes, the feature bins, the
   row index and the two int64 fixed-point values per row;
 - dtb_gbdt_leaves rows/s for the fitted trees (100 at the defaults);
@@ -82,14 +82,14 @@ def main():
     label = np.asarray(yt)
     gbm.Booster(dict(p, n_estimators=2), 'binary', 2, enc.feat_col, edges, dev).fit(cat, cont, label)   # warm-up
     booster = gbm.Booster(p, 'binary', 2, enc.feat_col, edges, dev)
-    booster.timer = {}
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     trees = booster.fit(cat, cont, label)
     torch.cuda.synchronize()
     res['fit_s'] = time.perf_counter() - t0
     res['trees'] = trees.n_trees
-    stages = {k: sum(s.elapsed_time(e) for s, e in v) / 1e3 for k, v in booster.timer.items()}
+    stages = {}
+    booster.fit(cat, cont, label, stages=stages)
     res['fit_stages_s'] = stages
     res['fit_host_and_sync_s'] = res['fit_s'] - sum(stages.values())
 
