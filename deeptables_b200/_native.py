@@ -143,6 +143,11 @@ _SIGNATURES = {
     'dtb_gradshap_reduce': (c_int, [P, P, P, P, P, P, P, c_int, P, P, c_int64, c_int, c_int, P, P, P, P]),
     'dtb_gradshap_means': (c_int, [P, c_int64, c_int, c_int, P, P]),
     'dtb_gradshap_output_grad': (c_int, [P, c_int64, c_int, c_int, c_int, P, P]),
+    'dtb_probe_loss_grad': (c_int, [P, c_int64, P, P, c_int64, c_int, c_int, c_int, c_int, P, P]),
+    'dtb_probe_tile_rows': (c_int, [c_int, c_int]),
+    'dtb_probe_join': (c_int, [P, c_int64, c_int, P, P]),
+    'dtb_probe_predict': (c_int, [P, c_int64, P, c_int64, c_int, c_int, c_int, P, P, P]),
+    'dtb_probe_correct': (c_int, [P, P, c_int64, P, P]),
     'dtb_te_remap': (c_int, [P, P, c_int64, c_int, P, P]),
     'dtb_te_keys': (c_int, [P, P, P, c_int64, c_int, c_int, c_int, P, P]),
     'dtb_te_segment_starts': (c_int, [P, c_int64, c_int64, P, P]),

@@ -49,6 +49,7 @@ class _Scope:
         self.frozen = False
         self.capture = None                # set of layer names whose outputs `apply` wants
         self.outputs = {}
+        self.layer_widths = {}
         self.anchor = torch.zeros(1, dtype=torch.float32, device=self.device, requires_grad=True)
         self._counters = {}
         self._indices = {}
@@ -132,6 +133,9 @@ class _Scope:
             self._prefix.pop()
 
     def record_output(self, name, out):
+        if not self.frozen:                # the build's dry run names every layer and gives its width
+            shape = getattr(out, 'shape', None)
+            self.layer_widths[name] = math.prod(shape[1:]) if shape is not None else None
         if self.capture is not None and name in self.capture:
             self.outputs[name] = out
 
@@ -1125,30 +1129,49 @@ class DeepModel:
             raise RuntimeError('model is not built: call fit() or load a model first')
         cat, cont = self._to_device_inputs(X)
         n = _length(X)
+        if capture:
+            return [o.cpu().numpy() for o in self.captured_outputs(cat, cont, n, batch_size, capture)]
         steps = math.ceil(n / batch_size)
         outs = []
-        captured = {k: [] for k in (capture or [])}
         for step in range(steps):
             lo = step * batch_size
             bc = cat[lo:lo + batch_size] if cat is not None else None
             bx = cont[lo:lo + batch_size] if cont is not None else None
-            if capture:
-                if bc is not None:
-                    self._catch_up(bc, self._step)
-                with torch.no_grad():
-                    self._forward(bc, bx, training=False, capture=set(capture))
-                for k in capture:
-                    if k not in self._scope.outputs:
-                        raise ValueError(f'No layer found in the model:{k}')
-                    o = self._scope.outputs[k]
-                    captured[k].append(L._materialize(o).detach())
-            else:
-                outs.append(self.predict_step(bc, bx))
+            outs.append(self.predict_step(bc, bx))
         if self.table is not None:
             self.table.check_status()
-        if capture:
-            return [torch.cat(captured[k]).cpu().numpy() for k in capture]
         return torch.cat(outs).cpu().numpy()
+
+    def captured_outputs(self, cat, cont, n, batch_size, capture):
+        """The outputs of the layers named in ``capture`` over the first ``n`` rows of the device inputs ``cat`` /
+        ``cont`` (either may be None), ``batch_size`` rows per inference forward: one device tensor per name, in order.
+        Embedding rows the lazy optimiser left behind are brought up to date first."""
+        captured = {k: [] for k in capture}
+        for lo in range(0, n, batch_size):
+            bc = cat[lo:lo + batch_size] if cat is not None else None
+            bx = cont[lo:lo + batch_size] if cont is not None else None
+            if bc is not None:
+                self._catch_up(bc, self._step)
+            with torch.no_grad():
+                self._forward(bc, bx, training=False, capture=set(capture))
+            for k in capture:
+                if k not in self._scope.outputs:
+                    raise ValueError(f'No layer found in the model:{k}')
+                o = self._scope.outputs[k]
+                captured[k].append(L._materialize(o).detach())
+        if self.table is not None:
+            self.table.check_status()
+        return [torch.cat(captured[k]) for k in capture]
+
+    def layer_widths(self):
+        """The layers ``apply`` can capture, name -> values per row (None when the layer's output has no shape): every
+        layer the model's forward records, and ``flatten_embeddings`` when it has categorical columns."""
+        if self.model is None:
+            raise RuntimeError('model is not built: call fit() or load a model first')
+        widths = dict(self._scope.layer_widths)
+        if self.n_fields:
+            widths.setdefault('flatten_embeddings', int(sum(self.emb_dims)))
+        return widths
 
     def apply(self, X, output_layers=[], concat_outputs=False, batch_size=128, verbose=0, transformer=None):
         """Outputs of named intermediate layers (reference deepmodel.py:143-163)."""

@@ -564,3 +564,16 @@ class DeepTable:
                                         model_file=os.path.join(filepath, f"{meta['model_name']}.npz"))
             dt._DeepTable__current_model = model      # the .npz carries the Adam step and moments (DeepModel._restore_optimizer)
         return dt
+
+
+def probe_evaluate(dt, X, y, X_test, y_test, layers, score_fn={}, *, batch_size=65536):
+    """How much of the label a linear model reads off each named layer (reference deeptable.py ``probe_evaluate``).
+
+    For each name in ``layers``, in order, the layer's outputs for ``X`` (flattened to ``(rows, -1)``) fit a
+    ``LogisticRegression(random_state=0)`` of scikit-learn 1.9 on ``dt.preprocessor.transform_y(y)``, computed on the
+    GPU (probe.py), and the probe is scored on ``X_test`` / ``y_test``.  Returns ``{layer: {'accuracy': mean
+    accuracy}}`` when ``score_fn`` is empty, else ``{layer: {name: fn(y_test, .)}}`` in ``score_fn`` order, where ``fn``
+    gets ``predict_proba[:, 1]`` when it is ``sklearn.metrics.roc_auc_score`` and the predicted classes otherwise.
+    ``batch_size`` rows go through each inference forward.  Binary and multiclass models only."""
+    from . import probe
+    return probe.probe_evaluate(dt, X, y, X_test, y_test, layers, score_fn, batch_size=batch_size)

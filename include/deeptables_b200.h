@@ -449,6 +449,30 @@ int dtb_gradshap_output_grad(const float* z, int64_t rows, int cols, int k, int 
 int dtb_pdp_block_sums(const float* prob, const double* weight, int64_t groups, int rows_per_group, int cols,
                        int block_rows, double* out, void* stream);
 
+/* ---- linear probes (deeptables_b200/probe.py; reference deeptable.py probe_evaluate) ------------------------------ */
+/* The objective of scikit-learn's lbfgs LogisticRegression over the float32 features X [n, d] (row stride ldx floats)
+ * with class codes y [n] and float64 weights W [K, d + 1] (column d: the intercept, read only when fit_intercept):
+ * z_k = sum_j x_j W[k, j] (+ W[k, d]).  Binary (K = 1, y in {0, 1}): loss log(1 + e^z) - y z, residual sigma(z) - y.
+ * Multinomial (K = classes, y in [0, K)): loss logsumexp(z) - z_y, residual softmax(z)_k - [k = y].
+ * partials [ceil(n / DTB_PROBE_BLOCK_ROWS), 1 + K (d + 1)] (float64) receives, per block of DTB_PROBE_BLOCK_ROWS rows,
+ * the sum of the losses, then sum r_k x_j at 1 + k (d + 1) + j (x_d = 1; 0 without an intercept).  Every sum runs over
+ * the block's rows in order, so a block's partial is the same bits for every tile_rows in [1, dtb_probe_tile_rows]
+ * (0: that most).  X is read once; every product and sum is float64. */
+#define DTB_PROBE_BLOCK_ROWS 1024
+#define DTB_PROBE_MAX_CLASSES 64
+int dtb_probe_loss_grad(const float* X, int64_t ldx, const int32_t* y, const double* W, int64_t n, int d, int K,
+                        int fit_intercept, int tile_rows, double* partials, void* stream);
+/* The most rows of d columns a loss_grad tile stages for K classes; 0 when a row does not fit in shared memory. */
+int dtb_probe_tile_rows(int d, int K);
+/* out[c] = partials[0, c] + partials[1, c] + ... in block order (out [width] float64). */
+int dtb_probe_join(const double* partials, int64_t blocks, int width, double* out, void* stream);
+/* The fitted probe on X [n, d]: proba [n, max(K, 2)] float64 (binary: [1 - sigma(z), sigma(z)]; multinomial: softmax)
+ * and codes [n]: binary z > 0, multinomial the first arg-max of z. */
+int dtb_probe_predict(const float* X, int64_t ldx, const double* W, int64_t n, int d, int K, int fit_intercept,
+                      double* proba, int32_t* codes, void* stream);
+/* *count += the number of rows i with pred[i] == truth[i] (an integer count; the caller zeroes *count). */
+int dtb_probe_correct(const int32_t* pred, const int32_t* truth, int64_t n, unsigned long long* count, void* stream);
+
 /* ---- target encoding (deeptables_b200/target_encoding.py; reference preprocessing/utils.py) ---------------------- */
 /* A column's rows carry a category code (-1: unknown), a fold id in [0, folds) and, for class targets, a class index
  * in [0, classes).  A continuous target has classes = 0.  Group g of a column's statistics is every fold (g = 0) or,
